@@ -1,16 +1,20 @@
 #!/usr/bin/env python
-"""bench.py -- denoised frames/sec of the Hallo denoising hot path on B200 (contract: see the task prompt).
+"""bench.py -- denoised frames/sec of the Hallo denoising hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--size 64] [--frames 16]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--size 64] [--frames 16] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
-A "step" is one denoising step of one 16-frame window at 512x512 (BASELINE.json configs[1]): UNet3D forward on
+A "step" is one denoising step of one 16-frame window at 512x512: UNet3D forward on
 the CFG batch (2, 4, 16, 64, 64) + CFG combine + DDIM update, fp16 storage / fp32 accumulate, random-init weights,
 synthetic inputs.  metric = 16 frames / (40 steps x time per step).  N > 1: the window is sharded over
 (CFG half x frame group) ranks (strong scaling); the temporal K/V all-gather and the CFG exchange are inside the
 timed region.  Timing: CUDA events around exactly K graph replays, barrier + synchronize on both sides, max over
-ranks.  The per-step activation working set (several GB) is far larger than the 126 MB L2, so no explicit flush
+ranks.  The per-step activation working set (several GB) is far larger than the 50 MB L2, so no explicit flush
 is needed between steps.
+
+--dump-outputs DIR writes the latents the last timed step produced, for the whole window (gathered over the ranks),
+to DIR/latents.npy (float32).  Weights and inputs
+are drawn from fixed seeds, so two builds run with the same arguments can be compared output for output.
 
 --impl reference and the `cpu_baseline` object of the default run time the reference's algorithm on the host cores
 through the oracle restatement (oracle/port.py, fp32, pinned to the unmodified reference at 1.7e-6): `cpu_baseline` is
@@ -38,15 +42,12 @@ N_DDIM = 40
 
 
 def load_peaks():
-    try:
-        p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        return dict(burst=p["bf16_tflops"], sustained=p["bf16_tflops_sustained"], hbm=p["hbm_gbs"], src="measured")
-    except Exception:
-        return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, src="fallback")
+    """H100 SXM data-sheet rates (dense fp16/bf16, HBM3) for a card allowed 700 W; a power-limited card reaches less."""
+    return dict(burst=989.0, sustained=989.0, hbm=3350.0, src="H100 SXM data sheet, dense, 700 W")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -220,7 +221,7 @@ def run_clip(args, rank, world, dev, dt, config):
             phases[k] = phases.get(k, 0.0) + v / len(anim.window_timings)
     eng = unet.engine(args.size, args.size, cl, pipe._window_shard(cl))
     if rank == 0:
-        line = {"metric": "end-to-end frames/sec, sliding 16-frame windows with 2 motion-frame overlap (BASELINE.json configs[4])",
+        line = {"metric": "end-to-end frames/sec, sliding 16-frame windows with 2 motion-frame overlap",
                 "value": video.shape[1] / dt_s, "unit": UNIT, "n_gpus": world, "windows": n_win, "frames": int(video.shape[1]),
                 "seconds": dt_s, "higher_is_better": True, "dtype": args.dtype, "data": "synthetic",
                 "config": {"workload": f"{n_win} windows x {cl} frames at {W}x{H}, {N_DDIM} DDIM steps, host in -> host out; "
@@ -306,7 +307,7 @@ def main():
     ap.add_argument("--frames", type=int, default=16)
     ap.add_argument("--dtype", default="f16", choices=["f16", "bf16"], help="storage / tensor-core input type (configs[3]: bf16)")
     ap.add_argument("--windows", type=int, default=0, metavar="N",
-                    help="BASELINE.json configs[4]: end-to-end frames/s of N sliding 16-frame windows through the whole "
+                    help="end-to-end frames/s of N sliding 16-frame windows through the whole "
                          "pipeline (VAE, ReferenceNet, conditioning, denoising, decode, motion-frame hand-off), host to host")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
@@ -317,10 +318,15 @@ def main():
     ap.add_argument("--kineto", default="", metavar="FILE",
                     help="after the timed run, trace 3 graph replays with torch.profiler (CUPTI) and write the per-kernel "
                          "in-graph durations and the idle gaps between kernels to FILE (diagnostic, not a bench value)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the latents of the last timed step (whole window) to DIR/latents.npy (float32)")
     ap.add_argument("--emulate-shard", type=int, default=0, metavar="R",
                     help="single GPU: run the workload of ONE rank of an R-rank job (cond half, first frame group, no "
                          "collectives) -- for ncu / op profiles of the sharded shapes; the JSON line is marked invalid")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.windows > 0 or args.emulate_shard > 1):
+        ap.error("--dump-outputs writes the latents of the timed denoising steps of the whole window; it does not "
+                 "apply to --impl reference, --windows or --emulate-shard")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -329,7 +335,7 @@ def main():
     config = {"workload": f"{args.size * 8}x{args.size * 8}, {args.frames}-frame window, CFG batch 2, "
                           f"{N_DDIM}-step DDIM ({which})", "latent": [2, 4, args.frames, args.size, args.size],
               "parallelism": f"frame-shard (both CFG halves per rank) over {world} rank(s)",
-              "l2": "per-step working set >> 126 MB L2, no explicit flush"}
+              "l2": "per-step working set >> 50 MB L2, no explicit flush"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -367,10 +373,14 @@ def main():
     torch.set_num_threads(max(1, host_threads() // world))
     try:
         sd = synth_state_dict_device(cfg, dev, seed=0)   # random-init weights, drawn on the GPU (identical on every rank)
+        config["weights"] = "seed 0, drawn on the device"
     except Exception as e:                               # set-up only: same distributions from the host streams
+        if args.dump_outputs:                            # other weights: the dumped outputs would not be comparable
+            raise
         print(f"# rank {rank}: on-device weight synthesis failed ({type(e).__name__}: {e}); drawing on the host", file=sys.stderr)
         from hallo_b200.synth import synth_state_dict
         sd = synth_state_dict(cfg, seed=0)
+        config["weights"] = "seed 0, drawn on the host (on-device synthesis failed)"
     W = PackedWeights(sd, cfg, dev, dt)
     del sd
     inp = synth_inputs(cfg, args.size, args.size, args.frames, seed=42)
@@ -382,10 +392,9 @@ def main():
         shard = Shard(halves=halves, frames=frames_, emulate_group=args.emulate_shard)
         config["emulated_rank_of"] = args.emulate_shard
     eng = DenoiseEngine(W, args.size, args.size, args.frames, shard)
-    # record the kernel-selection switches this line was measured with (defaults = the kernels that won their hardware A/B runs)
+    # record the kernel-selection switches this line was measured with
     try:
-        config["switches"] = {n: lib.get_option(n) for n in ("gemm_tepi", "gemm_1cta", "gemm_fill", "attn_occ2", "attn_poly",
-                                                              "attn_v1", "xattn_tc", "tattn_mma", "gn_fused")}
+        config["switches"] = {n: lib.get_option(n) for n in ("xattn_tc", "tattn_mma", "gn_fused", "gemm_splitk", "pdl")}
     except Exception:
         pass
     if world > 1:
@@ -482,6 +491,17 @@ def main():
     e1.record()
     barrier()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs:
+        lat = eng.latents.float()
+        if world > 1:                                    # ranks own contiguous frame groups in rank order
+            import torch.distributed as dist
+            parts = [torch.empty_like(lat) for _ in range(world)]
+            dist.all_gather(parts, lat.contiguous())
+            lat = torch.cat(parts, dim=2)
+        if rank == 0:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "latents.npy"), lat.cpu().numpy())
     clk = clocks.stop() if rank == 0 else None
     ms_step = ms_total / K
     fps = args.frames / (N_DDIM * ms_step * 1e-3)
@@ -547,8 +567,8 @@ def main():
             eng.arena.close()
         dist.barrier()
         if eng.px and eng.arena is None:
-            # NCCL exchange captured into the CUDA graph: destroy_process_group() still blocks for minutes after the graph
-            # object is dropped (measured again in round 2: profiles/r2e_summary.txt, exit 124) -- leave hard, as round 1 did
+            # NCCL exchange captured into the CUDA graph: destroy_process_group() can block for minutes after the graph
+            # object is dropped -- leave hard
             sys.stdout.flush()
             sys.stderr.flush()
             os._exit(0)
@@ -583,16 +603,9 @@ def main():
     attn_ms = sum(ts) / len(ts)
     attn_flops = spatial_attention_flops(L0, C0, n_cond, Bl - n_cond)
     achieved = attn_flops / (attn_ms * 1e-3) / 1e12
-    traffic, traffic_src = None, None
-    try:   # dram__bytes_read.sum + dram__bytes_write.sum of this kernel from the committed ncu --set full capture
-        ns = [e for e in json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_summaries.json"))) if e["name"] == "attn"][0]
-        if args.size == 64 and Bl == 32 and args.dtype == "f16":
-            traffic, traffic_src = ns["traffic_bytes"], "profiles/r2_ncu_summaries.json (ncu --set full, same kernel and shape)"
-    except Exception:
-        pass
-    roofline = {"kernel": "attn2_tc_kernel<D=40> (spatial self-attention + in-kernel reference-KV concat, L0)",
+    roofline = {"kernel": "attn_tc_kernel<D=40> (spatial self-attention + in-kernel reference-KV concat, L0)",
                 "bound": "tensor", "achieved": achieved, "peak": peaks["burst"], "unit": "TFLOP/s",
-                "frac": achieved / peaks["burst"], "traffic": traffic, "traffic_source": traffic_src,
+                "frac": achieved / peaks["burst"],
                 "peak_source": f"bf16 burst, {peaks['src']}",
                 "ms_per_launch": attn_ms, "algorithmic_flops_per_launch": attn_flops,
                 "whole_step": {"achieved": fl["total"] * world / world / (ms_step * 1e-3) / 1e12 / world,
@@ -617,8 +630,8 @@ def main():
         for k, v in sorted(agg.items(), key=lambda kv: -kv[1][0]):
             print(f"#   {k:22s} {v[0]:9.3f} ms  {100 * v[0] / tot:5.1f} %  x{v[1]}", file=sys.stderr)
 
-    # second roofline the north star asks for: the L0 3x3 conv of the ResNet blocks (implicit GEMM on tcgen05), timed
-    # live like the attention kernel; informational (the graded `roofline` object stays the attention kernel)
+    # second roofline: the L0 3x3 conv of the ResNet blocks (implicit GEMM on wgmma), timed live like the attention
+    # kernel; informational
     roofline_conv = None
     try:
         hh = args.size

@@ -1,4 +1,4 @@
-"""`hallo` overlay package: makes the B200 engine a drop-in under the reference's own import paths.
+"""`hallo` overlay package: makes the H100 engine a drop-in under the reference's own import paths.
 
 scripts/inference.py:38-47 imports `hallo.animate.face_animate`, `hallo.models.{audio_proj, unet_3d, unet_2d_condition,
 face_locator, image_proj}`, `hallo.datasets.*`, `hallo.utils.*`.  This package sits FIRST on sys.path

@@ -1,2 +1,2 @@
-"""hallo_b200: B200-native (sm_100a) implementation of the Hallo denoising hot path."""
+"""hallo_b200: H100-native (sm_90a) implementation of the Hallo denoising hot path."""
 __version__ = "0.1.0"

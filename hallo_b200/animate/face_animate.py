@@ -1,4 +1,4 @@
-"""FaceAnimatePipeline -- the reference pipeline's call surface over the B200 denoising engine.
+"""FaceAnimatePipeline -- the reference pipeline's call surface over the H100 denoising engine.
 
 Mirrors hallo/animate/face_animate.py (FaceAnimatePipeline.__init__ :90-121, prepare_latents :136-188,
 decode_latents :222-246, __call__ :249-442): same constructor modules, same __call__ keywords and tensor
@@ -7,7 +7,7 @@ contracts, same RNG contract (CPU generator -> initial latents), same output obj
 
 What changed is who runs the 40-step loop (:384-427): instead of 40 x {torch.cat, UNet module walk, CFG,
 scheduler.step} this hands the window to hallo_b200.engine.DenoiseEngine, which replays one captured CUDA
-graph per step (UNet3D forward + CFG combine + DDIM update, all sm_100a kernels).  VAE, ReferenceNet,
+graph per step (UNet3D forward + CFG combine + DDIM update, all sm_90a kernels).  VAE, ReferenceNet,
 face_locator and image_proj are the caller's modules (outside the hot path, SURVEY.md 8f).
 """
 from __future__ import annotations

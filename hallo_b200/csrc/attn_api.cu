@@ -1,4 +1,4 @@
-// C entry point of hallo_b200_attention: picks the kernel generation per shape.
+// C entry point of hallo_b200_attention: picks the kernel instance per head dim.
 #include "host_common.cuh"
 #include <cstdlib>
 
@@ -6,30 +6,11 @@ namespace hb {
 
 template <typename T>
 static int dispatch_attn(const hb_attention_params* p, cudaStream_t s) {
-  const bool v1 = option(OPT_ATTN_V1) != 0;     // A/B switches (hallo_b200_set_option / HALLO_B200_ATTN_*)
-  const int poly = option(OPT_ATTN_POLY);
-  const int occ2 = option(OPT_ATTN_OCC2);        // head_dim 40: 64-key steps, two CTAs (four query tiles) per SM
+  // template arguments: head dim, K / V ring depth, CTAs per SM (registers: O grows with the head dim)
   switch (p->head_dim) {
-    // v2 (two query tiles per CTA, P in TMEM) when a frame has at least one full pair of tiles; the
-    // single-tile kernel otherwise (small L) and for head_dim 160 at small L.
-    case 40:
-      if (p->L >= 256 && !v1 && occ2 != 0) {
-        if (poly == 4) return launch_attn2<T, 40, 64, 4, 2>(p, s);
-        if (poly == 3) return launch_attn2<T, 40, 64, 3, 2>(p, s);
-        if (poly == 2) return launch_attn2<T, 40, 64, 2, 2>(p, s);
-        return launch_attn2<T, 40, 64, 0, 2>(p, s);
-      }
-      if (p->L >= 256 && !v1) {
-        if (poly == 4) return launch_attn2<T, 40, 128, 4>(p, s);
-        if (poly == 3) return launch_attn2<T, 40, 128, 3>(p, s);
-        if (poly == 2) return launch_attn2<T, 40, 128, 2>(p, s);
-        return launch_attn2<T, 40, 128, 0>(p, s);
-      }
-      return launch_attn<T, 40, 128, 2>(p, s);
-    case 80:
-      if (p->L >= 256 && !v1) return launch_attn2<T, 80, 128, 0>(p, s);
-      return launch_attn<T, 80, 64, 2>(p, s);
-    case 160: return launch_attn<T, 160, 64, 2>(p, s);   // 2 x (2 S buffers + O) does not fit TMEM at d = 160
+    case 40: return launch_attn<T, 40, 3, 2>(p, s);
+    case 80: return launch_attn<T, 80, 2, 1>(p, s);
+    case 160: return launch_attn<T, 160, 2, 1>(p, s);
     default: return fail(HB_ERR_BAD_SHAPE, "attention: head_dim %d not in {40, 80, 160}", p->head_dim);
   }
 }

@@ -880,10 +880,13 @@ static int groupnorm_impl(int dtype, const void* x1, int C1, const void* x2, int
     // one-launch path for slabs (HW x C/G halfs) that fit shared memory -- opt-in, see gn_fused_kernel
     const int cpg = C / G;
     const size_t slab = (size_t)HW * cpg * 2;
-    // measured (profiles/r2_first_call_summary.txt): the one-launch kernel wins where the three launches are pure
-    // latency -- levels 2-3 (HW <= 256), and any norm of a sharded rank whose whole input is a few MB -- and loses on
-    // the 40-80 MB norms of levels 0-1 at 32 frames (a CTA reads C/G-channel slivers of every pixel: 1.9 -> 3.7 ms)
-    const bool small = HW <= 256 || (size_t)N * HW * C * 2 <= ((size_t)12 << 20);
+    // A CTA of the one-launch kernel reads a C/G-channel sliver of every pixel, so it wins where the slivers are wide
+    // or the three launches are mostly latency.  Measured on an H100 SXM (80 GB, 400 W power limit), fp16, SiLU,
+    // three launches vs one, in us: HW <= 256 (levels 2-3): 60 vs 14 (N 32, HW 64, C 1280) up to 103 vs 51 (HW 256,
+    // C 2560); C/G = 40: 127 vs 104 (N 32, HW 1024, C 1280), 62 vs 23 at N 4; C/G = 20: 32 vs 20 at 5 MB (N 4, HW 1024,
+    // C 640) but 66 vs 97 at 40 MB; C/G = 10 (level 0, C 320): the one-launch kernel is slower at every size measured
+    // (5-80 MB, e.g. 30 vs 46 at N 4).
+    const bool small = HW <= 256 || cpg >= 40 || (cpg >= 20 && (size_t)N * HW * C * 2 <= ((size_t)12 << 20));
     if (hb::option(hb::OPT_GN_FUSED) != 0 && cpg % 2 == 0 && slab <= 96 * 1024 && sc.seg == 0 && small) {
       if (fpb_in <= 0) { fpb_in = N; fpb_out = N; frame_off = 0; }
       const int vw = (cpg % 8 == 0) ? 4 : ((cpg % 4 == 0) ? 2 : 1);     // channel pairs per access (16 / 8 / 4 bytes)
@@ -937,7 +940,7 @@ extern "C" int hallo_b200_cross_attention(int dtype, const void* Q, int64_t ldq,
     return fail(HB_ERR_BAD_SHAPE, "cross_attention: head_dim=%d n_keys=%d", head_dim, n_keys);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   {
-    // tensor-core path (csrc/xattn_tc.cu) for the layouts the engine produces; CUDA cores otherwise
+    // tensor-core path (csrc/attn_tc.cu) for the layouts the engine produces; CUDA cores otherwise
     const int r = hb::xattn_tc_try(dtype, Q, ldq, q_region_stride, K, V, ldkv, kv_region_stride, O, ldo, o_region_stride,
                                    frames, L, heads, head_dim, n_keys, kv_frame_div, regions, s);
     if (r <= 0) return r;

@@ -1,47 +1,38 @@
-// hallo_b200_gemm: persistent warp-specialised tcgen05 GEMM / implicit-GEMM conv3x3.
+// hallo_b200_gemm: persistent warp-specialised wgmma GEMM / implicit-GEMM conv3x3 (sm_90a).
 //
-//   warp 0      : TMA producer  (A tile 128x64, W tile BNx64 per stage, 128B-swizzled)
-//   warp 1      : MMA issuer    (one elected lane; tcgen05.mma M=128, N=BN, K=16; fp32 in TMEM)
-//   warps 2..9  : epilogue      (tcgen05.ld -> bias / temb / GEGLU / mask / residual -> global);
-//                 warp w drains TMEM lanes 32*(w%4).. and accumulator columns (w-2)/4 * BN/2 ..
+//   warps 0-3, 4-7 : two consumer warpgroups.  Warpgroup g owns rows [64g, 64g + 64) of the 128 x BN tile: one
+//                    wgmma m64nBNk16 per 16-wide K step (fp32 accumulators in registers), then the epilogue
+//                    (bias / temb / GEGLU / LayerNorm fold / mask / residual / row statistics) straight from the
+//                    accumulator registers to global memory.
+//   warp 8         : TMA producer (A tile 128x64, W tile BNx64 per stage, 128B-swizzled), one elected lane.
 //
-// Two TMEM accumulator stages let the MMA of tile i+1 overlap the epilogue of tile i.
+// Each warpgroup keeps one wgmma group in flight: the stage of K step i is handed back to the producer once the
+// MMAs of step i + 1 have been issued and those of step i have completed.
 //
 // Split-K (p.splits = S > 1, chosen by the host when the tiles cover less than half of the SMs): the grid holds one
-// CTA (pair) per (tile, split); split s runs k-blocks [s*kper, (s+1)*kper).  Splits 1.. store their raw fp32
-// accumulators to the workspace ([tile][split-1][pair rank][column][row]: coalesced along rows) and bump one counter
-// per (tile, rank, epilogue warp); split 0 waits for S-1 arrivals on the counter of each of its epilogue warps, adds
-// the partials in split order and runs the usual epilogue.  All CTAs of such a grid are co-resident (<= 1 per SM),
-// so the wait cannot deadlock; the summation order is fixed, so results do not depend on timing.
+// CTA per (tile, split); split s runs k-blocks [s*kper, (s+1)*kper).  Splits 1.. store their raw fp32 accumulators to
+// the workspace ([tile][split-1][register][thread]: coalesced) and bump one counter per (tile, warpgroup); split 0
+// waits for S-1 arrivals on the counter of each of its warpgroups, adds the partials in split order and runs the
+// usual epilogue.  All CTAs of such a grid are co-resident (<= 1 per SM), so the wait cannot deadlock; the
+// summation order is fixed, so results do not depend on timing.
 // Tiles are walked n-fastest so the CTAs running concurrently share the same A rows in L2.
 //
 // Implicit conv: the A operand of tap (kh,kw) is the NHWC box shifted by (kh-1, kw-1); TMA's
 // out-of-bounds zero fill supplies the padding, so no im2col buffer exists anywhere.
-//
-// CG = 2 (CTA pair, tcgen05 cta_group::2): two CTAs of a cluster own a 256 x BN tile.  Each CTA stages its own
-// 128 A rows and HALF of the W rows, the leader issues one M=256 MMA per K step for both SMs and multicasts its
-// commits.  A single-CTA M=128 x N=160 MMA needs 9 KB of operand reads per 80 cycles on top of the TMA fill of the
-// same stage (~225 B/clk against a ~128 B/clk shared-memory port): measured 2x below the tensor-pipe rate
-// (profiles/r1_launches_v3_summary.txt).  Sharing W across the pair and widening BN to 192/256 brings the
-// shared-memory traffic back under the port limit.
 #include <cstdlib>
 
 #include "host_common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace hb {
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;
-constexpr int kGemmThreads = 320;   // TMA warp, MMA warp, 8 epilogue warps (2 per TMEM lane quarter)
-constexpr int kStgStride = 80;   // bytes per staged row: 64 B of data + 16 B pad (conflict-free 128-bit access)
-
-template <typename T>
-__device__ __forceinline__ void load8g(const T* p, float (&v)[8]) {
-  const uint4 u = *reinterpret_cast<const uint4*>(p);
-  const float2 a = Cvt<T>::unpack2(u.x), b = Cvt<T>::unpack2(u.y), c = Cvt<T>::unpack2(u.z), d = Cvt<T>::unpack2(u.w);
-  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y; v[4] = c.x; v[5] = c.y; v[6] = d.x; v[7] = d.y;
-}
+constexpr int kBN = 160;              // divides every channel count of the UNet (320, 640, 1280, ...)
+constexpr int kGemmStages = 6;
+constexpr int kGemmThreads = 288;     // two consumer warpgroups + the TMA warp
+constexpr int kGemmConsumers = 256;
 
 struct GemmDev {
   int M, N, K, K1;
@@ -61,41 +52,13 @@ struct GemmDev {
   const float* ln_colsum;
   float ln_eps;
   float* stats_out;
-  hb_row_scatter sc;   // sc.seg > 0: output rows go to peer buffers (direct epilogue only)
-  int splits;          // split-K factor S (1 = off); S > 1 => gridDim.x == tiles * S * CG
+  hb_row_scatter sc;   // sc.seg > 0: output rows go to peer buffers
+  int splits;          // split-K factor S (1 = off); S > 1 => gridDim.x == tiles * S
   float* ws;           // S > 1: fp32 partial tiles
-  int* cnt;            // S > 1: arrival counters, [tile][rank][epilogue warp], zero between launches
+  int* cnt;            // S > 1: arrival counters, [tile][warpgroup], zero between launches
   // conv geometry
   int cin, img_n, img_h, img_w, box_w, box_h, box_n, tiles_w, tiles_h, stride2;
 };
-
-// Timeline tracing (tools/gemm_trace.py builds a second library with -DHB_GEMM_TRACE): four recording threads per CTA
-// (TMA producer, MMA issuer, the elected thread of each epilogue group) append (event, index, clock64) records to a
-// global buffer set with hallo_b200_gemm_trace_buffer().  Compiles to nothing in the product library.
-#ifdef HB_GEMM_TRACE
-__device__ long long* g_gemm_trace = nullptr;
-constexpr int kTraceSlots = 256;                    // records per recorder
-struct Tracer {
-  long long* base;
-  int n;
-  __device__ Tracer(int recorder) {
-    base = g_gemm_trace ? g_gemm_trace + ((size_t)blockIdx.x * 4 + recorder) * (2 * kTraceSlots) : nullptr;
-    n = 0;
-  }
-  __device__ __forceinline__ void rec(int ev, int idx) {
-    if (base != nullptr && n < kTraceSlots) {
-      base[2 * n] = ((long long)ev << 32) | (unsigned)idx;
-      base[2 * n + 1] = clock64();
-      ++n;
-    }
-  }
-};
-#define HB_TRACE_DECL(name, recorder) Tracer name(recorder)
-#define HB_TRACE(name, ev, idx) name.rec(ev, idx)
-#else
-#define HB_TRACE_DECL(name, recorder)
-#define HB_TRACE(name, ev, idx)
-#endif
 
 // split-K: wait until `need` partial tiles have been published on *cnt, then re-arm the counter for the next launch
 __device__ __forceinline__ void splitk_wait(int* cnt, int need) {
@@ -113,762 +76,300 @@ __device__ __forceinline__ void splitk_wait(int* cnt, int need) {
   *cnt = 0;
 }
 
-__device__ __forceinline__ void tmem_ld_cw(uint32_t taddr, uint32_t (&r)[16]) { tmem_ld_x16(taddr, r); }
-__device__ __forceinline__ void tmem_ld_cw(uint32_t taddr, uint32_t (&r)[32]) { tmem_ld_x32(taddr, r); }
-
-constexpr int kPanelCols = 32;                        // output columns per staged panel (TMA-store epilogue)
-constexpr int kPanelBytes = kBM * kPanelCols * 2;     // 128 rows x 64 B, CU_TENSOR_MAP_SWIZZLE_64B
-constexpr int kEpiBufs = 4;                           // panel buffers per warp group: store in flight | being written | 2 residuals landing
-                                                      // (3 buffers = residual requested 2 panels ahead, less than one HBM latency at K = 320:
-                                                      //  profiles/r2_ncu_summaries.json gemm_k320)
-
-template <int BN, int STAGES, int CG, bool TEPI = false>
+template <int BN, int STAGES>
 struct GemmSmem {
   static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kBBytes = (BN / CG) * kBK * 2;   // a CTA of a pair stages half of the W rows
+  static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStgOffset = STAGES * kStageBytes;                 // TEPI: 2 warp groups x kEpiBufs panel buffers
-  static constexpr int kBarOffset = kStgOffset + (TEPI ? 2 * kEpiBufs * kPanelBytes : 0);
+  static constexpr int kBarOffset = STAGES * kStageBytes;
   static constexpr int kTotal = kBarOffset + 256 + 1024;  // + barriers + alignment slack
   static_assert(kStageBytes % 1024 == 0, "stage alignment");
 };
 
-// TEPI: epilogue through shared memory and TMA.  The direct epilogue has every lane own one output ROW, so each
-// 16-byte store (and residual load) of a warp touches 32 different 128-byte lines: ~BN*16 LSU wavefronts per
-// tile for the stores and as many for the residual, against BN*K/32 clk of MMA -- the K <= 640 GEMMs that make
-// up most of the step are bound by it (cuBLAS is 1.25-1.5x faster on those shapes,
-// profiles/r1_kbench_gemm_staged_epilogue_regression.log).  With TEPI the two groups of 4 epilogue warps write
-// 128 x 32 output panels into swizzled shared memory (conflict-free), an elected thread stores each panel with
-// one cp.async.bulk.tensor (clipped at the tensor edge, so no row masks) and the residual panel is prefetched
-// by TMA into the same buffer two panels ahead.
-//
-// EPI (TEPI kernels only) fixes the epilogue at compile time: EPI_PLAIN = bias / group bias / row scale / residual,
-// EPI_GEGLU = the same with the (value, gate) GEGLU pairing, EPI_FULL = every option decided at run time (activation,
-// folded LayerNorm, row statistics).  One kernel with all options live is ~130 KB of SASS whose executed path hops over
-// the dead branches of four unrolled units: the epilogue warps then wait on instruction fetch ("no_inst" in
-// profiles/r2_ncu_gemm_k320_stalls.txt; 450 clk between two trace points with no work in between,
-// profiles/r2_gemm_trace_before.txt), and with K <= 640 the epilogue, not the MMA, sets the tile rate.
+// EPI fixes the epilogue at compile time: EPI_PLAIN = bias / group bias / row scale / residual, EPI_GEGLU = the same
+// with the (value, gate) GEGLU pairing, EPI_FULL = every option decided at run time (activation, folded LayerNorm,
+// row statistics).  The common cases then carry no dead branches in their epilogue.
 enum { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_FULL = 2 };
 
-template <typename T, int BN, int STAGES, bool CONV, int CG, bool TEPI = false, int EPI = EPI_FULL>
+template <typename T, int BN, int STAGES, bool CONV, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-               const __grid_constant__ CUtensorMap tmB, const GemmDev p,
-               const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR) {
-  using SM = GemmSmem<BN, STAGES, CG, TEPI>;
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
-  const int cta_stride = gridDim.x / CG;          // persistent loop stride in units of (pairs of) CTAs
-  const int cta_first = blockIdx.x / CG;
-  constexpr uint32_t kAccStride = 256;  // TMEM column offset between the two accumulator stages
-  static_assert(BN % 32 == 0 && BN <= 256, "BN");
-  static_assert(CG == 1 || CG == 2, "cta_group");
+               const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
+  using SM = GemmSmem<BN, STAGES>;
+  static_assert(BN % 16 == 0 && BN <= 256, "BN");
+  constexpr int R = BN / 2;             // accumulator registers per consumer thread
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* res_bar = tempty_bar + 2;      // TEPI: residual panel landed, [group][buffer]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + 2 * kEpiBufs);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], kGemmConsumers);
+    }
+    fence_barrier_init();
+  }
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (p.K1 < p.K) tma_prefetch_desc(&tmA2);
-    if (TEPI) {
-      tma_prefetch_desc(&tmC);
-      if (p.residual != nullptr) tma_prefetch_desc(&tmR);
-    }
   }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], CG);        // pair: leader's expect_tx arrive + the peer producer's remote arrive
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 8 * CG);  // pair: the epilogue warps of both CTAs release the leader's accumulator
-    }
-    if (TEPI)
-      for (int s = 0; s < 2 * kEpiBufs; ++s) mbar_init(&res_bar[s], 1);
-    fence_barrier_init();
-  }
-  if (warp == 2) {
-    if (CG == 2) tmem_alloc_cg2<512>(tmem_slot); else tmem_alloc<512>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  if (CG == 2) cluster_sync_all();        // peer barriers must be initialised before any remote arrive / multicast
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();        // everything above (barriers, TMEM, tensor-map prefetch) may overlap the predecessor's tail
+  pdl_wait();        // everything above (barriers, tensor-map prefetch) may overlap the predecessor's tail
   pdl_launch();
 
-  // a pair walks (pairs of) M tiles: tile t covers M tiles {CG*tm2, CG*tm2 + 1}; this CTA takes tm = CG*tm2 + rank
-  const int num_tiles = ((p.tiles_m + CG - 1) / CG) * p.tiles_n;
+  const int num_tiles = p.tiles_m * p.tiles_n;
   const int kblocks = p.K / kBK;
   const int cin_blocks = CONV ? p.cin / kBK : 1;
-  // split-K: CTA (pair) c owns unit (tile c / S, split c % S) and nothing else -> every tile loop below runs once
+  // split-K: CTA c owns unit (tile c / S, split c % S) and nothing else -> every tile loop below runs once
   const int S = p.splits;
-  const int split = S > 1 ? cta_first % S : 0;
-  const int first = S > 1 ? cta_first / S : cta_first;
-  const int stride = S > 1 ? num_tiles : cta_stride;
+  const int split = S > 1 ? (int)blockIdx.x % S : 0;
+  const int first = S > 1 ? (int)blockIdx.x / S : (int)blockIdx.x;
+  const int stride = S > 1 ? num_tiles : (int)gridDim.x;
   const int kper = (kblocks + S - 1) / S;
   const int kb0 = split * kper;
   const int kb1 = (kb0 + kper < kblocks) ? kb0 + kper : kblocks;
 
-  if (warp == 0) {
+  auto tile_origin = [&](int t, int& tm, int& tn, int& n0, int& h0, int& w0) {
+    tm = t / p.tiles_n;
+    tn = t % p.tiles_n;
+    n0 = h0 = w0 = 0;
+    if (CONV) {
+      const int per_img = p.tiles_w * p.tiles_h;
+      const int nb = tm / per_img;
+      const int rem = tm - nb * per_img;
+      const int hb_ = rem / p.tiles_w;
+      n0 = nb * p.box_n;
+      h0 = hb_ * p.box_h;
+      w0 = (rem - hb_ * p.tiles_w) * p.box_w;
+    }
+  };
+
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      HB_TRACE_DECL(tr, 0);
-      HB_TRACE(tr, 1, 0);
       for (int t = first; t < num_tiles; t += stride) {
-        const int tm = (t / p.tiles_n) * CG + (int)rank;
-        const int tn = t % p.tiles_n;
-        int n0 = 0, h0 = 0, w0 = 0;
-        HB_TRACE(tr, 2, t);
-        if (CONV) {
-          int per_img = p.tiles_w * p.tiles_h;
-          int nb = tm / per_img;
-          int rem = tm - nb * per_img;
-          int hb_ = rem / p.tiles_w;
-          int wb = rem - hb_ * p.tiles_w;
-          n0 = nb * p.box_n;
-          h0 = hb_ * p.box_h;
-          w0 = wb * p.box_w;
-        }
+        int tm, tn, n0, h0, w0;
+        tile_origin(t, tm, tn, n0, h0, w0);
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1, 0x11);
           uint8_t* sa = smem + stage * SM::kStageBytes;
           uint8_t* sb = sa + SM::kABytes;
-          if (CG == 2) {
-            if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * SM::kStageBytes);
-            else mbar_arrive_leader(&full_bar[stage]);
-          } else {
-            mbar_arrive_expect_tx(&full_bar[stage], SM::kStageBytes);
-          }
+          mbar_arrive_expect_tx(&full_bar[stage], SM::kStageBytes);
           if (CONV) {
-            int tap = kb / cin_blocks;
-            int cb = kb - tap * cin_blocks;
-            int kh = tap / 3, kw = tap - kh * 3;
+            const int tap = kb / cin_blocks;
+            const int cb = kb - tap * cin_blocks;
+            const int kh = tap / 3, kw = tap - kh * 3;
             if (p.stride2) {
               // input is stored as 4 phase planes [(p*2+q)*img_n + n][h/2][w/2][C] (x[2i+p][2j+q]);
               // tap kh reads phase (kh==1 ? 0 : 1) at row offset (kh==0 ? -1 : 0)
               const int ph = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
-              if (CG == 2) tma_load_4d_cg2(sa, &tmA, &full_bar[stage], cb * kBK, w0 - (kw == 0), h0 - (kh == 0),
-                                           (ph * 2 + pw) * p.img_n + n0);
-              else tma_load_4d(sa, &tmA, &full_bar[stage], cb * kBK, w0 - (kw == 0), h0 - (kh == 0),
-                               (ph * 2 + pw) * p.img_n + n0);
+              tma_load_4d(sa, &tmA, &full_bar[stage], cb * kBK, w0 - (kw == 0), h0 - (kh == 0),
+                          (ph * 2 + pw) * p.img_n + n0);
             } else {
-              if (CG == 2) tma_load_4d_cg2(sa, &tmA, &full_bar[stage], cb * kBK, w0 + kw - 1, h0 + kh - 1, n0);
-              else tma_load_4d(sa, &tmA, &full_bar[stage], cb * kBK, w0 + kw - 1, h0 + kh - 1, n0);
+              tma_load_4d(sa, &tmA, &full_bar[stage], cb * kBK, w0 + kw - 1, h0 + kh - 1, n0);
             }
           } else {
-            int k = kb * kBK;
+            const int k = kb * kBK;
             const CUtensorMap* ma = (k < p.K1) ? &tmA : &tmA2;
-            const int kk = (k < p.K1) ? k : k - p.K1;
-            if (CG == 2) tma_load_2d_cg2(sa, ma, &full_bar[stage], kk, tm * kBM);
-            else tma_load_2d(sa, ma, &full_bar[stage], kk, tm * kBM);
+            tma_load_2d(sa, ma, &full_bar[stage], (k < p.K1) ? k : k - p.K1, tm * kBM);
           }
-          if (CG == 2) tma_load_2d_cg2(sb, &tmB, &full_bar[stage], kb * kBK, tn * BN + (int)rank * (BN / 2));
-          else tma_load_2d(sb, &tmB, &full_bar[stage], kb * kBK, tn * BN);
+          tma_load_2d(sb, &tmB, &full_bar[stage], kb * kBK, tn * BN);
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
           }
         }
-        HB_TRACE(tr, 3, t);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = make_idesc_f16(kBM * CG, BN, Cvt<T>::kFmt, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    HB_TRACE_DECL(tr, 1);
-    if (leader)   // in a pair only the leader CTA issues MMAs (for both SMs)
-    for (int t = first; t < num_tiles; t += stride, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      if (lane == 0) HB_TRACE(tr, 10, t);
-      mbar_wait(&tempty_bar[as], aphase ^ 1, 0x21);
-      tc_fence_after();
-      if (lane == 0) HB_TRACE(tr, 11, t);
-      const uint32_t d_tmem = tmem_base + as * kAccStride;
-#ifdef HB_GEMM_TRACE
-      long long wsum = 0;
-#endif
-      for (int kb = kb0; kb < kb1; ++kb) {
-#ifdef HB_GEMM_TRACE
-        const long long w0 = clock64();
-#endif
-        mbar_wait(&full_bar[stage], phase, 0x22);
-        tc_fence_after();
-#ifdef HB_GEMM_TRACE
-        wsum += clock64() - w0;
-#endif
-        if (lane == 0) {
-          if (kb == kb0) HB_TRACE(tr, 12, t);
-          if (kb == kb1 - 1) {
-            HB_TRACE(tr, 13, t);
-            HB_TRACE(tr, 14, (int)wsum);
-          }
-          const uint32_t sa = smem_u32(smem + stage * SM::kStageBytes);
-          const uint32_t sb = sa + SM::kABytes;
-          const uint64_t adesc = make_desc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = make_desc_sw128(sb, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            // advance 32 B (16 halfs) along K inside the 128 B swizzle row: +2 in (addr >> 4)
-            if (CG == 2) umma_f16_ss_cg2(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, ((kb - kb0) | k) != 0);
-            else umma_f16_ss(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, ((kb - kb0) | k) != 0);
-          }
-          if (CG == 2) {
-            umma_commit_cg2_mc(&empty_bar[stage]);
-            if (kb == kb1 - 1) umma_commit_cg2_mc(&tfull_bar[as]);
-          } else {
-            umma_commit(&empty_bar[stage]);
-            if (kb == kb1 - 1) umma_commit(&tfull_bar[as]);
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (split != 0) {
-    // ===================== split-K partial: raw fp32 accumulators -> workspace =====================
-    // each warp stores exactly the (rows, columns) that the same warp of the reducing CTA reads back
-    const int quarter = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    const bool geglu = (EPI == EPI_GEGLU) || (EPI == EPI_FULL && (p.flags & HB_EPI_GEGLU) != 0);
-    constexpr int UW = TEPI ? 32 : (((BN / 2) % 32 == 0) ? 32 : 16);
-    const int panels = (geglu ? BN / 64 : BN / 32);
-    const int my_panels = (panels - grp + 1) / 2;
-    const int nunits = TEPI ? (geglu ? 2 * my_panels : my_panels) : BN / 2 / UW;
-    const int t = first;
-    mbar_wait(&tfull_bar[0], 0, 0x35);
-    tc_fence_after();
-    float* ws = p.ws + ((((size_t)t * (S - 1) + (split - 1)) * CG + rank) * BN) * kBM + quarter * 32 + lane;
-    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16);
-    for (int u = 0; u < nunits; ++u) {
-      const int col = TEPI ? (geglu ? (grp + 2 * (u >> 1)) * 64 + (u & 1) * 32 : (grp + 2 * u) * 32) : grp * (BN / 2) + u * UW;
-      uint32_t r[UW];
-      tmem_ld_cw(taddr + col, r);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < UW; ++j) __stcg(ws + (size_t)(col + j) * kBM, __uint_as_float(r[j]));
-    }
-    __threadfence();
-    __syncwarp();
-    if (lane == 0) atomicAdd(p.cnt + ((t * CG + (int)rank) * 8 + (warp - 2)), 1);
-  } else if (TEPI) {
-    // ===================== epilogue warps, shared-memory staged + TMA stores =====================
-    const int quarter = warp & 3;        // TMEM lane quarter this warp may access
-    const int grp = (warp - 2) >> 2;     // group of 4 warps; takes output panels grp, grp + 2, ...
-    const bool elected = (quarter == 0 && lane == 0);
-    const T* bias = reinterpret_cast<const T*>(p.bias);
-    const T* gbias = reinterpret_cast<const T*>(p.group_bias);
-    const T* rscale = reinterpret_cast<const T*>(p.row_scale);
-    const bool geglu = (EPI == EPI_GEGLU) || (EPI == EPI_FULL && (p.flags & HB_EPI_GEGLU) != 0);
-    const bool has_res = p.residual != nullptr;
-    // a unit = 32 accumulator columns (one TMEM load); a panel = 32 output columns = 1 unit (2 with GEGLU)
-    constexpr int kMaxUnits = (BN % 64 == 0) ? 2 * ((BN / 64 + 1) / 2) : (BN / 32 + 1) / 2;
-    const int panels = (geglu ? BN / 64 : BN / 32);
-    const int my_panels = (panels - grp + 1) / 2;
-    const int my_units = geglu ? 2 * my_panels : my_panels;
-    const int out_bn = geglu ? BN / 2 : BN;                      // output columns per tile
-    uint8_t* stg = smem + SM::kStgOffset + grp * (kEpiBufs * kPanelBytes);
-    uint64_t* res_full = res_bar + grp * kEpiBufs;
-    const int r_in_tile = quarter * 32 + lane;
-    // panel buffer = 128 rows of 64 B, CU_TENSOR_MAP_SWIZZLE_64B: 16-byte chunk c of row r sits at
-    // r*64 + ((c ^ ((r >> 1) & 3)) << 4); the 8 rows of a quarter-warp phase hit 8 different bank groups
-    const uint32_t row_off = (uint32_t)r_in_tile * 64u;
-    const uint32_t row_sw = ((uint32_t)r_in_tile >> 1) & 3u;
+    return;
+  }
 
-    auto tile_origin = [&](int t, int& tm, int& tn, int& n0, int& h0, int& w0) {
-      tm = (t / p.tiles_n) * CG + (int)rank;
-      tn = t % p.tiles_n;
-      n0 = h0 = w0 = 0;
-      if (CONV) {
-        const int per_img = p.tiles_w * p.tiles_h;
-        const int nb = tm / per_img;
-        const int rem = tm - nb * per_img;
-        const int hb_ = rem / p.tiles_w;
-        n0 = nb * p.box_n;
-        h0 = hb_ * p.box_h;
-        w0 = (rem - hb_ * p.tiles_w) * p.box_w;
-      }
-    };
-    // residual prefetch iterator (elected thread only): the next (tile, panel) of this group to request
-    int pf_t = first, pf_i = 0, pf_b = 0;
-    auto prefetch_residual = [&]() {
-      if (pf_t >= num_tiles) return;
-      int tm, tn, n0, h0, w0;
-      tile_origin(pf_t, tm, tn, n0, h0, w0);
-      const int ocol = tn * out_bn + (grp + 2 * pf_i) * kPanelCols;
-      mbar_arrive_expect_tx(&res_full[pf_b], kPanelBytes);
-      if (CONV) tma_load_4d(stg + pf_b * kPanelBytes, &tmR, &res_full[pf_b], ocol, w0, h0, n0);
-      else tma_load_2d(stg + pf_b * kPanelBytes, &tmR, &res_full[pf_b], ocol, tm * kBM);
-      if (++pf_b == kEpiBufs) pf_b = 0;
-      if (++pf_i == my_panels) {
-        pf_i = 0;
-        pf_t += stride;
-      }
-    };
-    // panel q of this group lives in buffer q % kEpiBufs.  At the end of panel q the elected thread issues
-    // store(q) and waits only until store(q-1) has been READ (issued a whole panel earlier), which frees buffer
-    // (q-1) % kEpiBufs for the residual of panel q + kEpiBufs - 1: the residual runs kEpiBufs - 1 panels ahead.
-    if (has_res && elected) {
-      for (int i = 0; i < kEpiBufs - 1; ++i) prefetch_residual();
-    }
-    __syncwarp();
+  // ===================== consumer warpgroups: MMA + epilogue =====================
+  const int wg = threadIdx.x >> 7;
+  const int ct = threadIdx.x;                            // 0..255
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile rows r0 and r0 + 8 of this thread
+  const int cq = 2 * (lane & 3);                         // column pair within each 8-column block
+  const T* bias = reinterpret_cast<const T*>(p.bias);
+  const T* gbias = reinterpret_cast<const T*>(p.group_bias);
+  const T* rscale = reinterpret_cast<const T*>(p.row_scale);
+  const T* resid = reinterpret_cast<const T*>(p.residual);
+  T* C = reinterpret_cast<T*>(p.C);
+  const bool geglu = (EPI == EPI_GEGLU) || (EPI == EPI_FULL && (p.flags & HB_EPI_GEGLU) != 0);
+  const int n_out = geglu ? (p.N >> 1) : p.N;
 
-    int b = 0;                            // buffer of the current panel
-    uint32_t bphase = 0;                  // parity of res_full[b] for the current round through the buffers
-    int it = 0;
-    HB_TRACE_DECL(tr, 2 + grp);
-    for (int t = first; t < num_tiles; t += stride, ++it) {
-      int tm, tn, n0, h0, w0;
-      tile_origin(t, tm, tn, n0, h0, w0);
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      long long row;
-      bool row_ok;
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[R];
+  for (int t = first; t < num_tiles; t += stride) {
+    int tm, tn, n0, h0, w0;
+    tile_origin(t, tm, tn, n0, h0, w0);
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase, 0x22);
+      const uint32_t sa = smem_u32(smem + stage * SM::kStageBytes) + wg * (64 * 128);
+      const uint32_t sb = smem_u32(smem + stage * SM::kStageBytes + SM::kABytes);
+      const uint64_t adesc = make_desc_sw128(sa, 16, 1024);
+      const uint64_t bdesc = make_desc_sw128(sb, 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBK / 16; ++k) Wgmma<BN, T>::ss(acc, adesc + 2 * k, bdesc + 2 * k, ((kb - kb0) | k) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_pin(acc);
+    if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+
+    if (split != 0) {
+      // ===================== split-K partial: raw fp32 accumulators -> workspace =====================
+      float* ws = p.ws + ((size_t)t * (S - 1) + (split - 1)) * (size_t)(BN * kBM) + ct;
+#pragma unroll
+      for (int j = 0; j < R; ++j) __stcg(ws + j * kGemmConsumers, acc[j]);
+      __threadfence();
+      named_bar_sync(1 + wg, 128);
+      if ((ct & 127) == 0) atomicAdd(p.cnt + 2 * t + wg, 1);
+      continue;
+    }
+    if (S > 1) {
+      if ((ct & 127) == 0) splitk_wait(p.cnt + 2 * t + wg, S - 1);
+      named_bar_sync(1 + wg, 128);
+      __threadfence();
+#pragma unroll 1
+      for (int s2 = 0; s2 < S - 1; ++s2) {
+        const float* w = p.ws + ((size_t)t * (S - 1) + s2) * (size_t)(BN * kBM) + ct;
+#pragma unroll
+        for (int j = 0; j < R; ++j) acc[j] += __ldcg(w + j * kGemmConsumers);
+      }
+    }
+
+    // ===================== epilogue: this thread's two rows, BN/4 columns each =====================
+    long long row[2];
+    bool row_ok[2];
+    float rs[2], ln_mu[2], ln_rstd[2], osum[2], osq[2];
+    const T* gb_row[2];
+    T* crow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r_in_tile = r0 + 8 * h;
       if (CONV) {
         const int dn = r_in_tile / (p.box_h * p.box_w);
         const int r2 = r_in_tile - dn * (p.box_h * p.box_w);
         const int dh = r2 / p.box_w;
         const int dw = r2 - dh * p.box_w;
         const int in_ = n0 + dn, ih = h0 + dh, iw = w0 + dw;
-        row = ((long long)in_ * p.img_h + ih) * p.img_w + iw;
-        row_ok = in_ < p.img_n && ih < p.img_h && iw < p.img_w;   // overhanging rows are clipped by the TMA store
+        row[h] = ((long long)in_ * p.img_h + ih) * p.img_w + iw;
+        row_ok[h] = in_ < p.img_n && ih < p.img_h && iw < p.img_w;   // boxes may overhang the image batch
       } else {
-        row = (long long)tm * kBM + r_in_tile;
-        row_ok = row < p.M;
+        row[h] = (long long)tm * kBM + r_in_tile;
+        row_ok[h] = row[h] < p.M;
       }
-      float rs = p.alpha;
-      if (rscale != nullptr && row_ok) rs *= Cvt<T>::to_f(rscale[row]);
-      const T* gb_row = nullptr;
-      if (gbias != nullptr && row_ok) gb_row = gbias + (row / p.rows_per_group) * p.ld_group_bias;
-      float ln_mu = 0.f, ln_rstd = 1.f;
-      if (EPI == EPI_FULL && p.ln_stats != nullptr && row_ok) {
-        const float2 st = *reinterpret_cast<const float2*>(p.ln_stats + 2 * row);
-        ln_mu = st.x / (float)p.K;
-        const float var = fmaxf(st.y / (float)p.K - ln_mu * ln_mu, 0.f);
-        ln_rstd = rsqrtf(var + p.ln_eps);
+      rs[h] = p.alpha;
+      if (rscale != nullptr && row_ok[h]) rs[h] *= Cvt<T>::to_f(rscale[row[h]]);
+      gb_row[h] = (gbias != nullptr && row_ok[h]) ? gbias + (row[h] / p.rows_per_group) * p.ld_group_bias : nullptr;
+      // folded LayerNorm of the A rows: v = rstd * (acc - mu * colsum[n])
+      ln_mu[h] = 0.f;
+      ln_rstd[h] = 1.f;
+      if (EPI == EPI_FULL && p.ln_stats != nullptr && row_ok[h]) {
+        const float2 st = *reinterpret_cast<const float2*>(p.ln_stats + 2 * row[h]);
+        ln_mu[h] = st.x / (float)p.K;
+        const float var = fmaxf(st.y / (float)p.K - ln_mu[h] * ln_mu[h], 0.f);
+        ln_rstd[h] = rsqrtf(var + p.ln_eps);
       }
-      float osum = 0.f, osq = 0.f;
-      // accumulator column of unit u: plain -> panel (grp + 2u); GEGLU -> panel (grp + 2(u/2)), half (u & 1)
-      auto unit_col = [&](int u) { return geglu ? (grp + 2 * (u >> 1)) * 64 + (u & 1) * 32 : (grp + 2 * u) * 32; };
-      // the per-column epilogue vectors of this warp's units do not depend on the accumulator: pull them into L1 while
-      // the MMAs run (lane u takes unit u; a unit is 64 B of bias / one 128 B line of column sums)
-      if (lane < my_units) {
-        const int pc = tn * BN + unit_col(lane);
-        if (bias != nullptr) prefetch_l1(bias + pc);
-        if (gb_row != nullptr) prefetch_l1(gb_row + pc);
-        if (EPI == EPI_FULL && p.ln_colsum != nullptr) prefetch_l1(p.ln_colsum + pc);
+      osum[h] = osq[h] = 0.f;
+      // destination of this row: local C, or (frame-sharded motion module) the owner rank's buffer
+      crow[h] = C + row[h] * p.ldc;
+      if (p.sc.seg > 0 && row_ok[h]) {
+        const long long sg = row[h] / p.sc.seg;
+        const long long qq = row[h] - sg * p.sc.seg;
+        const long long dd = sg / p.sc.segs_per_dest;
+        const long long ii = sg - dd * p.sc.segs_per_dest;
+        crow[h] = reinterpret_cast<T*>(p.sc.base[dd]) + (ii * p.sc.seg_stride + p.sc.row0 + qq) * p.ldc;
       }
-
-      if (elected) HB_TRACE(tr, 20, t);
-      mbar_wait(&tfull_bar[as], aphase, 0x31);
-      tc_fence_after();
-      if (elected) HB_TRACE(tr, 21, t);
-      const float* wsr = nullptr;          // split-K: partial tiles of splits 1.. for this lane's row
-      if (S > 1) {
-        if (lane == 0) splitk_wait(p.cnt + ((t * CG + (int)rank) * 8 + (warp - 2)), S - 1);
-        __threadfence();
-        __syncwarp();
-        wsr = p.ws + (((size_t)t * (S - 1)) * CG + rank) * BN * kBM + r_in_tile;
-      }
-      const uint32_t taddr = tmem_base + as * kAccStride + ((uint32_t)(quarter * 32) << 16);
-      uint32_t racc[2][32];
-      tmem_ld_x32(taddr + unit_col(0), racc[0]);
+    }
 #pragma unroll
-      for (int u = 0; u < kMaxUnits; ++u) {
-        if (u >= my_units) break;
-        tmem_ld_wait();
-        uint32_t(&r)[32] = racc[u & 1];
-        if (u + 1 < my_units) tmem_ld_x32(taddr + unit_col(u + 1), racc[(u + 1) & 1]);   // overlaps with the math below
-        const int acol0 = tn * BN + unit_col(u);                   // first accumulator (= weight row) column
-        const bool first_of_panel = !geglu || (u & 1) == 0;
-        const bool last_of_panel = !geglu || (u & 1) == 1;
-        uint8_t* sbuf = stg + b * kPanelBytes;
-        const uint32_t sbuf_u32 = smem_u32(sbuf);
-        if (first_of_panel && has_res) {
-          if (elected) HB_TRACE(tr, 22, u);
-          mbar_wait(&res_full[b], bphase, 0x33);
-          if (elected) HB_TRACE(tr, 23, u);
-        }
-
-        if (elected) HB_TRACE(tr, 27, u);
-        float v[32];
+    for (int i = 0; i < BN / 8; ++i) {
+      const int col = tn * BN + 8 * i + cq;         // accumulator (= weight row) column of acc[4i], acc[4i + 1]
+      if (col >= p.N) continue;                     // N % 8 == 0: col + 1 < N as well
+      float2 b2 = make_float2(0.f, 0.f), cs = make_float2(0.f, 0.f);
+      if (bias != nullptr) b2 = Cvt<T>::unpack2(*reinterpret_cast<const uint32_t*>(bias + col));
+      if (EPI == EPI_FULL && p.ln_stats != nullptr) cs = *reinterpret_cast<const float2*>(p.ln_colsum + col);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        if (S > 1) {
-#pragma unroll 1
-          for (int s2 = 0; s2 < S - 1; ++s2) {
-            const float* w = wsr + ((size_t)s2 * CG * BN + unit_col(u)) * kBM;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] += __ldcg(w + j * kBM);
-          }
-        }
+      for (int h = 0; h < 2; ++h) {
+        if (!row_ok[h]) continue;
+        float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
         if (EPI == EPI_FULL && p.ln_stats != nullptr) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 cs = *reinterpret_cast<const float4*>(p.ln_colsum + acol0 + j);
-            v[j + 0] = ln_rstd * (v[j + 0] - ln_mu * cs.x);
-            v[j + 1] = ln_rstd * (v[j + 1] - ln_mu * cs.y);
-            v[j + 2] = ln_rstd * (v[j + 2] - ln_mu * cs.z);
-            v[j + 3] = ln_rstd * (v[j + 3] - ln_mu * cs.w);
-          }
+          v0 = ln_rstd[h] * (v0 - ln_mu[h] * cs.x);
+          v1 = ln_rstd[h] * (v1 - ln_mu[h] * cs.y);
         }
-        if (bias != nullptr) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            float f[8];
-            load8g(bias + acol0 + j, f);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) v[j + k] += f[k];
-          }
+        v0 += b2.x;
+        v1 += b2.y;
+        if (gb_row[h] != nullptr) {
+          const float2 g2 = Cvt<T>::unpack2(*reinterpret_cast<const uint32_t*>(gb_row[h] + col));
+          v0 += g2.x;
+          v1 += g2.y;
         }
-        if (gb_row != nullptr) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            float f[8];
-            load8g(gb_row + acol0 + j, f);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) v[j + k] += f[k];
-          }
-        }
-        if (elected) HB_TRACE(tr, 28, u);
         if (EPI == EPI_FULL) {
           if (p.flags & HB_EPI_SILU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = silu_f(v[j]);
+            v0 = silu_f(v0);
+            v1 = silu_f(v1);
           } else if (p.flags & HB_EPI_RELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+            v0 = fmaxf(v0, 0.f);
+            v1 = fmaxf(v1, 0.f);
           }
         }
         if (geglu) {
-          // (value, gate) pairs: 32 accumulator columns -> 16 outputs = chunks 2*(u&1), 2*(u&1)+1 of the panel row
-          float o[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) o[j] = v[2 * j] * gelu_fast(v[2 * j + 1]) * rs;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const uint32_t cell = sbuf_u32 + row_off + ((((uint32_t)((u & 1) * 2 + c)) ^ row_sw) << 4);
-            if (has_res) {
-              const uint4 rv = lds128(cell);
-              const float2 a0 = Cvt<T>::unpack2(rv.x), a1 = Cvt<T>::unpack2(rv.y), a2 = Cvt<T>::unpack2(rv.z),
-                           a3 = Cvt<T>::unpack2(rv.w);
-              o[c * 8 + 0] += a0.x; o[c * 8 + 1] += a0.y; o[c * 8 + 2] += a1.x; o[c * 8 + 3] += a1.y;
-              o[c * 8 + 4] += a2.x; o[c * 8 + 5] += a2.y; o[c * 8 + 6] += a3.x; o[c * 8 + 7] += a3.y;
-            }
-            uint4 o4;
-            o4.x = Cvt<T>::pack2(o[c * 8 + 0], o[c * 8 + 1]);
-            o4.y = Cvt<T>::pack2(o[c * 8 + 2], o[c * 8 + 3]);
-            o4.z = Cvt<T>::pack2(o[c * 8 + 4], o[c * 8 + 5]);
-            o4.w = Cvt<T>::pack2(o[c * 8 + 6], o[c * 8 + 7]);
-            sts128(cell, o4);
+          // (value, gate) pair -> one output column
+          const int oc = col >> 1;
+          float o = v0 * gelu_fast(v1) * rs[h];
+          if (resid != nullptr) o += Cvt<T>::to_f(resid[row[h] * p.ldr + oc]);
+          crow[h][oc] = Cvt<T>::from_f(o);
+        } else if (col < n_out) {
+          float w0 = v0 * rs[h], w1 = v1 * rs[h];
+          if (resid != nullptr) {
+            const float2 r2 = Cvt<T>::unpack2(*reinterpret_cast<const uint32_t*>(resid + row[h] * p.ldr + col));
+            w0 += r2.x;
+            w1 += r2.y;
           }
-        } else {
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const uint32_t cell = sbuf_u32 + row_off + ((((uint32_t)c) ^ row_sw) << 4);
-            float w[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) w[k] = v[c * 8 + k] * rs;
-            if (has_res) {
-              const uint4 rv = lds128(cell);
-              const float2 a0 = Cvt<T>::unpack2(rv.x), a1 = Cvt<T>::unpack2(rv.y), a2 = Cvt<T>::unpack2(rv.z),
-                           a3 = Cvt<T>::unpack2(rv.w);
-              w[0] += a0.x; w[1] += a0.y; w[2] += a1.x; w[3] += a1.y;
-              w[4] += a2.x; w[5] += a2.y; w[6] += a3.x; w[7] += a3.y;
-            }
-            uint4 o4;
-            o4.x = Cvt<T>::pack2(w[0], w[1]);
-            o4.y = Cvt<T>::pack2(w[2], w[3]);
-            o4.z = Cvt<T>::pack2(w[4], w[5]);
-            o4.w = Cvt<T>::pack2(w[6], w[7]);
-            sts128(cell, o4);
-            if (EPI == EPI_FULL && p.stats_out != nullptr) {
-              // statistics of the values as the next LayerNorm will read them (rounded to the storage type)
-              const float2 q0 = Cvt<T>::unpack2(o4.x), q1 = Cvt<T>::unpack2(o4.y), q2 = Cvt<T>::unpack2(o4.z),
-                           q3 = Cvt<T>::unpack2(o4.w);
-              osum += (q0.x + q0.y) + (q1.x + q1.y) + (q2.x + q2.y) + (q3.x + q3.y);
-              osq += (q0.x * q0.x + q0.y * q0.y) + (q1.x * q1.x + q1.y * q1.y) + (q2.x * q2.x + q2.y * q2.y) +
-                     (q3.x * q3.x + q3.y * q3.y);
-            }
+          const uint32_t o2 = Cvt<T>::pack2(w0, w1);
+          *reinterpret_cast<uint32_t*>(crow[h] + col) = o2;
+          if (EPI == EPI_FULL && p.stats_out != nullptr) {
+            // statistics of the values as the next LayerNorm will read them (rounded to the storage type)
+            const float2 q = Cvt<T>::unpack2(o2);
+            osum[h] += q.x + q.y;
+            osq[h] += q.x * q.x + q.y * q.y;
           }
         }
-        if (last_of_panel) {
-          if (elected) HB_TRACE(tr, 24, u);
-          fence_proxy_async_smem();                       // generic-proxy writes -> visible to the TMA store
-          named_bar_sync(1 + grp, 128);
-          if (elected) {
-            HB_TRACE(tr, 25, u);
-            const int ocol = tn * out_bn + (geglu ? (grp + 2 * (u >> 1)) : (grp + 2 * u)) * kPanelCols;
-            if (CONV) tma_store_4d(&tmC, sbuf, ocol, w0, h0, n0);
-            else tma_store_2d(&tmC, sbuf, ocol, tm * kBM);
-            bulk_commit_group();
-            bulk_wait_group_read<1>();                    // the previous panel's buffer is free again ...
-            HB_TRACE(tr, 26, u);
-            if (has_res) prefetch_residual();             // ... and takes the residual of panel q + kEpiBufs - 1
-          }
-          __syncwarp();
-          if (++b == kEpiBufs) {
-            b = 0;
-            bphase ^= 1u;
-          }
-        }
-      }
-      if (EPI == EPI_FULL && p.stats_out != nullptr && row_ok) {
-        atomicAdd(p.stats_out + 2 * row, osum);
-        atomicAdd(p.stats_out + 2 * row + 1, osq);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CG == 2 && !leader) mbar_arrive_leader(&tempty_bar[as]);
-        else mbar_arrive(&tempty_bar[as]);
       }
     }
-    // the staging buffers must outlive the READS of the last stores; their global writes complete with the grid
-    if (elected) bulk_wait_group_read<0>();
-  } else {
-    // ===================== epilogue warps =====================
-    const int quarter = warp & 3;  // TMEM lane quarter this warp may access
-    const T* bias = reinterpret_cast<const T*>(p.bias);
-    const T* gbias = reinterpret_cast<const T*>(p.group_bias);
-    const T* rscale = reinterpret_cast<const T*>(p.row_scale);
-    const T* resid = reinterpret_cast<const T*>(p.residual);
-    T* C = reinterpret_cast<T*>(p.C);
-    const bool geglu = (EPI == EPI_GEGLU) || (EPI == EPI_FULL && (p.flags & HB_EPI_GEGLU) != 0);
-    const int chalf = (warp - 2) >> 2;   // which half of the accumulator columns this warp drains
-    int it = 0;
-    for (int t = first; t < num_tiles; t += stride, ++it) {
-      const int tm = (t / p.tiles_n) * CG + (int)rank;
-      const int tn = t % p.tiles_n;
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      const int r_in_tile = quarter * 32 + lane;
-      long long row;
-      bool row_ok;
-      if (CONV) {
-        int per_img = p.tiles_w * p.tiles_h;
-        int nb = tm / per_img;
-        int rem = tm - nb * per_img;
-        int hb_ = rem / p.tiles_w;
-        int wb = rem - hb_ * p.tiles_w;
-        int dn = r_in_tile / (p.box_h * p.box_w);
-        int r2 = r_in_tile - dn * (p.box_h * p.box_w);
-        int dh = r2 / p.box_w;
-        int dw = r2 - dh * p.box_w;
-        const int in_ = nb * p.box_n + dn, ih = hb_ * p.box_h + dh, iw = wb * p.box_w + dw;
-        row = ((long long)in_ * p.img_h + ih) * p.img_w + iw;
-        row_ok = in_ < p.img_n && ih < p.img_h && iw < p.img_w;   // boxes may overhang the image batch
-      } else {
-        row = (long long)tm * kBM + r_in_tile;
-        row_ok = row < p.M;
-      }
-      float rs = p.alpha;
-      if (rscale != nullptr && row_ok) rs *= Cvt<T>::to_f(rscale[row]);
-      const T* gb_row = nullptr;
-      if (gbias != nullptr && row_ok) gb_row = gbias + (row / p.rows_per_group) * p.ld_group_bias;
-      const int n_out = geglu ? (p.N >> 1) : p.N;
-      // folded LayerNorm of the A rows: v = rstd * (acc - mu * colsum[n])
-      float ln_mu = 0.f, ln_rstd = 1.f;
-      if (EPI == EPI_FULL && p.ln_stats != nullptr && row_ok) {
-        const float2 st = *reinterpret_cast<const float2*>(p.ln_stats + 2 * row);
-        ln_mu = st.x / (float)p.K;
-        const float var = fmaxf(st.y / (float)p.K - ln_mu * ln_mu, 0.f);
-        ln_rstd = rsqrtf(var + p.ln_eps);
-      }
-      float osum = 0.f, osq = 0.f;
-      // destination of this lane's output row: local C, or (frame-sharded motion module) the owner rank's buffer
-      T* crow = C + row * p.ldc;
-      if (p.sc.seg > 0 && row_ok) {
-        const long long sg = row / p.sc.seg;
-        const long long qq = row - sg * p.sc.seg;
-        const long long dd = sg / p.sc.segs_per_dest;
-        const long long ii = sg - dd * p.sc.segs_per_dest;
-        crow = reinterpret_cast<T*>(p.sc.base[dd]) + (ii * p.sc.seg_stride + p.sc.row0 + qq) * p.ldc;
-      }
-      // epilogue vectors of this warp's BN/2 columns -> L1 while the MMAs run (one lane per 64 B)
-      {
-        const int pc = tn * BN + chalf * (BN / 2) + lane * 32;
-        if (lane * 32 < BN / 2 && pc < p.N) {
-          if (bias != nullptr) prefetch_l1(bias + pc);
-          if (gb_row != nullptr) prefetch_l1(gb_row + pc);
-          if (EPI == EPI_FULL && p.ln_colsum != nullptr) {
-            prefetch_l1(p.ln_colsum + pc);
-            if (pc + 16 < p.N) prefetch_l1(p.ln_colsum + pc + 16);
-          }
+    if (EPI == EPI_FULL && p.stats_out != nullptr) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        // the four lanes of a quad hold the same row
+        osum[h] += __shfl_xor_sync(0xffffffffu, osum[h], 1);
+        osum[h] += __shfl_xor_sync(0xffffffffu, osum[h], 2);
+        osq[h] += __shfl_xor_sync(0xffffffffu, osq[h], 1);
+        osq[h] += __shfl_xor_sync(0xffffffffu, osq[h], 2);
+        if ((lane & 3) == 0 && row_ok[h]) {
+          atomicAdd(p.stats_out + 2 * row[h], osum[h]);
+          atomicAdd(p.stats_out + 2 * row[h] + 1, osq[h]);
         }
-      }
-
-      mbar_wait(&tfull_bar[as], aphase, 0x31);
-      tc_fence_after();
-      const float* wsr = nullptr;          // split-K: partial tiles of splits 1.. for this lane's row
-      if (S > 1) {
-        if (lane == 0) splitk_wait(p.cnt + ((t * CG + (int)rank) * 8 + (warp - 2)), S - 1);
-        __threadfence();
-        __syncwarp();
-        wsr = p.ws + (((size_t)t * (S - 1)) * CG + rank) * BN * kBM + r_in_tile;
-      }
-      // this warp owns TMEM lanes [32*quarter, +32) and accumulator columns [chalf*BN/2, +BN/2), CW at a time
-      // (CW = 32 when the half-tile allows it: more independent work per TMEM load for the GELU epilogue)
-      const uint32_t taddr = tmem_base + as * kAccStride + ((uint32_t)(quarter * 32) << 16) + chalf * (BN / 2);
-      constexpr int CW = ((BN / 2) % 32 == 0) ? 32 : 16;
-      constexpr int kChunks = BN / 2 / CW;
-      uint32_t racc[2][CW];
-      tmem_ld_cw(taddr, racc[0]);
-      tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c) {
-        uint32_t(&r)[CW] = racc[c & 1];
-        if (c + 1 < kChunks) tmem_ld_cw(taddr + (c + 1) * CW, racc[(c + 1) & 1]);   // overlaps with this chunk's math
-        const int col0 = tn * BN + chalf * (BN / 2) + c * CW;
-        if (row_ok && col0 < p.N) {
-          float v[CW];
-#pragma unroll
-          for (int j = 0; j < CW; ++j) v[j] = __uint_as_float(r[j]);
-          if (S > 1) {
-#pragma unroll 1
-            for (int s2 = 0; s2 < S - 1; ++s2) {
-              const float* w = wsr + ((size_t)s2 * CG * BN + chalf * (BN / 2) + c * CW) * kBM;
-#pragma unroll
-              for (int j = 0; j < CW; ++j) v[j] += __ldcg(w + j * kBM);
-            }
-          }
-          if (EPI == EPI_FULL && p.ln_stats != nullptr) {
-#pragma unroll
-            for (int j = 0; j < CW; j += 4) {
-              if (col0 + j < p.N) {
-                const float4 cs = *reinterpret_cast<const float4*>(p.ln_colsum + col0 + j);
-                v[j + 0] = ln_rstd * (v[j + 0] - ln_mu * cs.x);
-                v[j + 1] = ln_rstd * (v[j + 1] - ln_mu * cs.y);
-                v[j + 2] = ln_rstd * (v[j + 2] - ln_mu * cs.z);
-                v[j + 3] = ln_rstd * (v[j + 3] - ln_mu * cs.w);
-              }
-            }
-          }
-          if (bias != nullptr) {
-#pragma unroll
-            for (int j = 0; j < CW; j += 8) {
-              if (col0 + j < p.N) {
-                float f[8];
-                load8g(bias + col0 + j, f);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) v[j + q] += f[q];
-              }
-            }
-          }
-          if (gb_row != nullptr) {
-#pragma unroll
-            for (int j = 0; j < CW; j += 8) {
-              if (col0 + j < p.N) {
-                float f[8];
-                load8g(gb_row + col0 + j, f);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) v[j + q] += f[q];
-              }
-            }
-          }
-          if (EPI == EPI_FULL && (p.flags & HB_EPI_SILU)) {
-#pragma unroll
-            for (int j = 0; j < CW; ++j) v[j] = silu_f(v[j]);
-          } else if (EPI == EPI_FULL && (p.flags & HB_EPI_RELU)) {
-#pragma unroll
-            for (int j = 0; j < CW; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-          if (geglu) {
-            // (value, gate) pairs: CW accumulator columns -> CW/2 outputs
-            const int ocol0 = col0 >> 1;
-            float o[CW / 2];
-#pragma unroll
-            for (int j = 0; j < CW / 2; ++j) o[j] = v[2 * j] * gelu_fast(v[2 * j + 1]) * rs;
-#pragma unroll
-            for (int j = 0; j < CW / 2; j += 8) {
-              if (resid != nullptr) {
-                float f[8];
-                load8g(resid + row * p.ldr + ocol0 + j, f);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) o[j + q] += f[q];
-              }
-              uint4 o4;
-              o4.x = Cvt<T>::pack2(o[j + 0], o[j + 1]);
-              o4.y = Cvt<T>::pack2(o[j + 2], o[j + 3]);
-              o4.z = Cvt<T>::pack2(o[j + 4], o[j + 5]);
-              o4.w = Cvt<T>::pack2(o[j + 6], o[j + 7]);
-              *reinterpret_cast<uint4*>(crow + ocol0 + j) = o4;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < CW; j += 8) {
-              if (col0 + j < n_out) {
-                float w[8];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) w[q] = v[j + q] * rs;
-                if (resid != nullptr) {
-                  float f[8];
-                  load8g(resid + row * p.ldr + col0 + j, f);
-#pragma unroll
-                  for (int q = 0; q < 8; ++q) w[q] += f[q];
-                }
-                uint4 o4;
-                o4.x = Cvt<T>::pack2(w[0], w[1]);
-                o4.y = Cvt<T>::pack2(w[2], w[3]);
-                o4.z = Cvt<T>::pack2(w[4], w[5]);
-                o4.w = Cvt<T>::pack2(w[6], w[7]);
-                *reinterpret_cast<uint4*>(crow + col0 + j) = o4;
-                if (EPI == EPI_FULL && p.stats_out != nullptr) {
-                  // statistics of the values as the next LayerNorm will read them (rounded to the storage type)
-                  const float2 q0 = Cvt<T>::unpack2(o4.x), q1 = Cvt<T>::unpack2(o4.y), q2 = Cvt<T>::unpack2(o4.z),
-                               q3 = Cvt<T>::unpack2(o4.w);
-                  osum += (q0.x + q0.y) + (q1.x + q1.y) + (q2.x + q2.y) + (q3.x + q3.y);
-                  osq += (q0.x * q0.x + q0.y * q0.y) + (q1.x * q1.x + q1.y * q1.y) + (q2.x * q2.x + q2.y * q2.y) +
-                         (q3.x * q3.x + q3.y * q3.y);
-                }
-              }
-            }
-          }
-        }
-        __syncwarp();
-        if (c + 1 < kChunks) tmem_ld_wait();
-      }
-      if (EPI == EPI_FULL && p.stats_out != nullptr && row_ok) {
-        atomicAdd(p.stats_out + 2 * row, osum);
-        atomicAdd(p.stats_out + 2 * row + 1, osq);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CG == 2 && !leader) mbar_arrive_leader(&tempty_bar[as]);
-        else mbar_arrive(&tempty_bar[as]);
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (CG == 2) cluster_sync_all();        // the peer may still be arriving on / reading this CTA's shared memory
-  if (warp == 2) {
-    tc_fence_after();
-    if (CG == 2) tmem_dealloc_cg2<512>(tmem_base); else tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -876,7 +377,7 @@ constexpr long long kSplitKCounterBytes = 8192;     // head of the split-K works
 constexpr int kSplitKMinBlocks = 32;                // shortest K loop (64-wide k-blocks) that is split
 static int g_last_splits = 1;                       // split factor of the most recent launch (tests / diagnostics)
 
-// Split factor of a launch of `tiles` (pairs of) tiles on `max_ctas` (pairs of) SMs; pure host arithmetic, also exported
+// Split factor of a launch of `tiles` tiles (of cta-group `cg`) on `max_ctas` SMs; pure host arithmetic, also exported
 // as hallo_b200_gemm_choose_splits for the CPU tests.  1 = unsplit.
 static int choose_splits(int tiles, int max_ctas, int kblocks, int cg, int bn, long long workspace_bytes, int splitk_opt) {
   const int min_blocks = splitk_opt > 1 ? splitk_opt : kSplitKMinBlocks;
@@ -911,9 +412,9 @@ static void pick_conv_box(int n, int h, int w, int* bw, int* bh, int* bn) {
     }
 }
 
-template <typename T, int BN, int STAGES, int CG, bool TEPI = false, int EPI = EPI_FULL>
+template <typename T, int BN, int STAGES, int EPI>
 static int launch_gemm(const hb_gemm_params* q, cudaStream_t stream) {
-  using SM = GemmSmem<BN, STAGES, CG, TEPI>;
+  using SM = GemmSmem<BN, STAGES>;
   static_assert(SM::kTotal <= 232448, "gemm smem budget");
   GemmDev d{};
   d.M = q->M;
@@ -943,7 +444,7 @@ static int launch_gemm(const hb_gemm_params* q, cudaStream_t stream) {
   {
     uint64_t dims[2] = {(uint64_t)q->K, (uint64_t)q->N};
     uint64_t str[1] = {(uint64_t)q->ldw * 2};
-    uint32_t box[2] = {kBK, (uint32_t)(BN / CG)};
+    uint32_t box[2] = {kBK, (uint32_t)BN};
     if ((rc = make_tmap_16b(&tmB, q->dtype, q->W, 2, dims, str, box)) != HB_OK) return rc;
   }
   if (q->conv3x3) {
@@ -987,50 +488,26 @@ static int launch_gemm(const hb_gemm_params* q, cudaStream_t stream) {
     }
   }
 
-  // output / residual maps of the TMA-store epilogue: 128-row x 32-column panels (conv: the same NHWC box as A)
-  CUtensorMap tmC = tmA, tmR = tmA;
-  if (TEPI) {
-    const uint64_t n_out = (q->flags & HB_EPI_GEGLU) ? (uint64_t)q->N / 2 : (uint64_t)q->N;
-    for (int which = 0; which < 2; ++which) {
-      const void* base = which == 0 ? q->C : q->residual;
-      const uint64_t ld = which == 0 ? (uint64_t)q->ldc : (uint64_t)q->ldr;
-      if (base == nullptr) continue;
-      CUtensorMap* out = which == 0 ? &tmC : &tmR;
-      if (q->conv3x3) {
-        uint64_t dims[4] = {n_out, (uint64_t)q->img_w, (uint64_t)q->img_h, (uint64_t)q->img_n};
-        uint64_t str[3] = {ld * 2, ld * 2 * q->img_w, ld * 2 * q->img_w * q->img_h};
-        uint32_t box[4] = {kPanelCols, (uint32_t)d.box_w, (uint32_t)d.box_h, (uint32_t)d.box_n};
-        if ((rc = make_tmap_16b(out, q->dtype, base, 4, dims, str, box, 64)) != HB_OK) return rc;
-      } else {
-        uint64_t dims[2] = {n_out, (uint64_t)q->M};
-        uint64_t str[1] = {ld * 2};
-        uint32_t box[2] = {kPanelCols, kBM};
-        if ((rc = make_tmap_16b(out, q->dtype, base, 2, dims, str, box, 64)) != HB_OK) return rc;
-      }
-    }
-  }
-
-  const int tiles = ((d.tiles_m + CG - 1) / CG) * d.tiles_n;      // (pairs of) tiles
+  const int tiles = d.tiles_m * d.tiles_n;
   if (tiles <= 0) return HB_OK;
-  const int max_ctas = num_sms() / CG;
-  // split-K: a CTA streams kblocks/S operand stages (32 KB each) and the reducing CTA reads S-1 partial tiles
-  // (128 x BN fp32) back, so the per-CTA traffic is smallest near S = sqrt(kblocks / 4).  The hand-over (partial
-  // store, fence, counter, read-back) costs ~4 us, which a K loop below kSplitKMinBlocks k-blocks does not win back
-  // (profiles/r2_kbench_latency_splitk.log); an option value > 1 overrides that threshold (A/B runs).
-  d.splits = choose_splits(tiles, max_ctas, q->K / kBK, CG, BN, q->workspace != nullptr ? q->workspace_bytes : 0,
+  const int max_ctas = num_sms();
+  // split-K: a CTA streams kblocks/S operand stages and the reducing CTA reads S-1 partial tiles (128 x BN fp32)
+  // back, so the per-CTA traffic is smallest near S = sqrt(kblocks / 4).  The hand-over (partial store, fence,
+  // counter, read-back) costs a few microseconds, which a K loop below kSplitKMinBlocks k-blocks does not win back;
+  // an option value > 1 overrides that threshold (A/B runs).
+  d.splits = choose_splits(tiles, max_ctas, q->K / kBK, 1, BN, q->workspace != nullptr ? q->workspace_bytes : 0,
                            option(OPT_GEMM_SPLITK));
   if (d.splits > 1) {
     d.cnt = reinterpret_cast<int*>(q->workspace);
     d.ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(q->workspace) + kSplitKCounterBytes);
   }
   g_last_splits = d.splits;
-  const int grid = (d.splits > 1 ? tiles * d.splits : (tiles < max_ctas ? tiles : max_ctas)) * CG;
-  // instantiated: GEMM with every epilogue (PLAIN, GEGLU on TEPI kernels, FULL = all options at run time); conv3x3
-  // with PLAIN only (hallo_b200_gemm rejects an activation / LayerNorm fold / GEGLU on a conv)
-  constexpr bool kConvOk = (EPI == EPI_PLAIN);
-  auto kern = gemm_tc_kernel<T, BN, STAGES, false, CG, TEPI, EPI>;
-  if constexpr (kConvOk) {
-    if (q->conv3x3) kern = gemm_tc_kernel<T, BN, STAGES, true, CG, TEPI, EPI>;
+  const int grid = d.splits > 1 ? tiles * d.splits : (tiles < max_ctas ? tiles : max_ctas);
+  // instantiated: GEMM with every epilogue; conv3x3 with PLAIN only (hallo_b200_gemm rejects an activation /
+  // LayerNorm fold / GEGLU on a conv)
+  auto kern = gemm_tc_kernel<T, BN, STAGES, false, EPI>;
+  if constexpr (EPI == EPI_PLAIN) {
+    if (q->conv3x3) kern = gemm_tc_kernel<T, BN, STAGES, true, EPI>;
   } else {
     if (q->conv3x3) return fail(HB_ERR_BAD_SHAPE, "internal: conv3x3 routed to a GEMM-only epilogue");
   }
@@ -1039,63 +516,25 @@ static int launch_gemm(const hb_gemm_params* q, cudaStream_t stream) {
     HB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal));
     attr_set[q->conv3x3 ? 1 : 0] = true;
   }
-  HB_CUDA_CHECK(launch_kernel_cluster(kern, dim3(grid), dim3(kGemmThreads), SM::kTotal, stream, CG, tmA, tmA2, tmB, d, tmC, tmR));
+  HB_CUDA_CHECK(launch_kernel(kern, dim3(grid), dim3(kGemmThreads), SM::kTotal, stream, tmA, tmA2, tmB, d));
   HB_LAUNCH_CHECK();
   return HB_OK;
 }
 
 template <typename T>
 static int dispatch_gemm(const hb_gemm_params* p, cudaStream_t s) {
-  const bool force1 = option(OPT_GEMM_1CTA) != 0;     // A/B switch for benchmarking
-  const int tiles_m = p->conv3x3 ? 2 : (p->M + kBM - 1) / kBM;
   // anything beyond bias / group bias / row scale / residual: the epilogue with every option decided at run time
-  const bool plain = (p->flags & (HB_EPI_SILU | HB_EPI_RELU | HB_EPI_GEGLU)) == 0 && p->ln_stats == nullptr && p->stats_out == nullptr;
-  if (force1 || tiles_m < 2) return plain ? launch_gemm<T, 160, 5, 1, false, EPI_PLAIN>(p, s) : launch_gemm<T, 160, 5, 1>(p, s);
-  // TMA-store epilogue (TEPI): written after the last GPU session of round 1 -> opt-in until tests/test_gemm_gpu.py
-  // has passed with gemm_tepi = 1 on hardware.  Needs whole N tiles and 16-byte aligned C / residual.
-  const bool tepi_env = option(OPT_GEMM_TEPI) != 0;
-  const bool aligned = ((reinterpret_cast<uintptr_t>(p->C) | reinterpret_cast<uintptr_t>(p->residual)) & 15) == 0;
-  if (tepi_env && aligned && p->scatter == nullptr) {
-    const bool geglu = (p->flags & HB_EPI_GEGLU) != 0;
-    // activation / folded LayerNorm / row statistics: the epilogue with every option live (plain GEMMs only)
-    const bool full = (p->flags & (HB_EPI_SILU | HB_EPI_RELU)) != 0 || p->ln_stats != nullptr || p->stats_out != nullptr;
-    if (!full && geglu) {
-      if (p->N % 256 == 0) return launch_gemm<T, 256, 5, 2, true, EPI_GEGLU>(p, s);
-      if (p->N % 192 == 0) return launch_gemm<T, 192, 5, 2, true, EPI_GEGLU>(p, s);
-    } else if (!full) {
-      if (p->N % 256 == 0) return launch_gemm<T, 256, 5, 2, true, EPI_PLAIN>(p, s);
-      if (p->N % 192 == 0) return launch_gemm<T, 192, 5, 2, true, EPI_PLAIN>(p, s);
-      if (p->N % 160 == 0) return launch_gemm<T, 160, 6, 2, true, EPI_PLAIN>(p, s);
-    } else {
-      if (p->N % 256 == 0) return launch_gemm<T, 256, 5, 2, true>(p, s);
-      if (p->N % 192 == 0) return launch_gemm<T, 192, 5, 2, true>(p, s);
-      if (p->N % 160 == 0 && !geglu) return launch_gemm<T, 160, 6, 2, true>(p, s);
-    }
-  }
-  // option gemm_fill (opt-in, untested on hardware): when the widest N tile leaves SM pairs idle (small M: the
-  // per-rank shapes of a sharded window, levels 2-3), trade shared-memory efficiency for occupancy with BN 128 / 64
-  if (option(OPT_GEMM_FILL) != 0) {
-    const long long rows = p->conv3x3 ? (long long)p->img_n * p->img_h * p->img_w : (long long)p->M;
-    const long long tiles_m2 = ((rows + kBM - 1) / kBM + 1) / 2;
-    const int pairs = num_sms() / 2;
-    const int wide = p->N % 256 == 0 ? 256 : (p->N % 192 == 0 ? 192 : 160);
-    if (tiles_m2 * ((p->N + wide - 1) / wide) < pairs) {
-      if (p->N % 128 == 0 && tiles_m2 * (p->N / 128) >= pairs)
-        return plain ? launch_gemm<T, 128, 8, 2, false, EPI_PLAIN>(p, s) : launch_gemm<T, 128, 8, 2>(p, s);
-      if (p->N % 64 == 0) return plain ? launch_gemm<T, 64, 8, 2, false, EPI_PLAIN>(p, s) : launch_gemm<T, 64, 8, 2>(p, s);
-      if (p->N % 128 == 0) return plain ? launch_gemm<T, 128, 8, 2, false, EPI_PLAIN>(p, s) : launch_gemm<T, 128, 8, 2>(p, s);
-    }
-  }
-  // widest N tile that divides N: fewer shared-memory bytes per MMA flop (see the header comment)
-  if (p->N % 256 == 0) return plain ? launch_gemm<T, 256, 6, 2, false, EPI_PLAIN>(p, s) : launch_gemm<T, 256, 6, 2>(p, s);
-  if (p->N % 192 == 0) return plain ? launch_gemm<T, 192, 7, 2, false, EPI_PLAIN>(p, s) : launch_gemm<T, 192, 7, 2>(p, s);
-  return plain ? launch_gemm<T, 160, 7, 2, false, EPI_PLAIN>(p, s) : launch_gemm<T, 160, 7, 2>(p, s);
+  const bool geglu = (p->flags & HB_EPI_GEGLU) != 0;
+  const bool full = (p->flags & (HB_EPI_SILU | HB_EPI_RELU)) != 0 || p->ln_stats != nullptr || p->stats_out != nullptr;
+  if (full) return launch_gemm<T, kBN, kGemmStages, EPI_FULL>(p, s);
+  if (geglu) return launch_gemm<T, kBN, kGemmStages, EPI_GEGLU>(p, s);
+  return launch_gemm<T, kBN, kGemmStages, EPI_PLAIN>(p, s);
 }
 
 }  // namespace hb
 
 extern "C" long long hallo_b200_gemm_workspace_bytes(void) {
-  // counters + one 128 x 256 fp32 partial tile for every CTA of a 160-SM grid
+  // counters + 256 partial tiles of 128 x 160 fp32 (a split grid has at most one CTA per SM)
   return hb::kSplitKCounterBytes + 160LL * 256 * hb::kBM * (long long)sizeof(float);
 }
 
@@ -1104,14 +543,6 @@ extern "C" int hallo_b200_gemm_choose_splits(int tiles, int sm_units, int K, int
                                              int option_value) {
   return hb::choose_splits(tiles, sm_units, K / hb::kBK, cta_group, bn, workspace_bytes, option_value);
 }
-
-#ifdef HB_GEMM_TRACE
-// tools/gemm_trace.py only: buffer of gridDim.x * 4 recorders * 256 records * 2 int64 (NULL = off)
-extern "C" int hallo_b200_gemm_trace_buffer(void* buf) {
-  long long* p = reinterpret_cast<long long*>(buf);
-  return cudaMemcpyToSymbol(hb::g_gemm_trace, &p, sizeof(p)) == cudaSuccess ? 0 : -1;
-}
-#endif
 
 extern "C" int hallo_b200_gemm(const hb_gemm_params* p, hb_stream_t stream) {
   using namespace hb;
@@ -1138,7 +569,6 @@ extern "C" int hallo_b200_gemm(const hb_gemm_params* p, hb_stream_t stream) {
   if (p->A2 != nullptr && (p->K1 % kBK != 0 || p->K1 <= 0 || p->K1 >= p->K || p->conv3x3))
     return fail(HB_ERR_BAD_SHAPE, "hallo_b200_gemm: bad K split %d of %d", p->K1, p->K);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  // 160 divides every channel count of the UNet (320, 640, 1280, ...), so N tiles are never ragged.
   if (p->dtype == HB_F16) return dispatch_gemm<__half>(p, s);
   if (p->dtype == HB_BF16) return dispatch_gemm<__nv_bfloat16>(p, s);
   return fail(HB_ERR_BAD_DTYPE, "hallo_b200_gemm: dtype %d", p->dtype);

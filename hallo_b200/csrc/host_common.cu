@@ -10,10 +10,10 @@ namespace hb {
 char g_last_error[512] = "";
 std::atomic<int64_t> g_launch_count{0};
 
-static const char* const kOptionNames[OPT_COUNT] = {"gemm_tepi", "gemm_1cta", "attn_occ2", "attn_poly", "attn_v1", "xattn_tc", "tattn_mma", "gemm_fill", "gn_fused", "gemm_splitk", "pdl"};
-// defaults: the kernels promoted after their round-2 hardware runs (profiles/r2_first_call_*) are ON; setting an
-// option to 0 selects the previous-generation kernel (A/B measurements, shapes the new kernel does not cover)
-static const int kOptionDefaults[OPT_COUNT] = {1, 0, 1, 0, 0, 1, 1, 1, 1, 1, 0};
+static const char* const kOptionNames[OPT_COUNT] = {"xattn_tc", "tattn_mma", "gn_fused", "gemm_splitk", "pdl"};
+// defaults: the tensor-core / fused kernels are ON; setting an option to 0 selects the CUDA-core or unfused kernel
+// (A/B measurements).  pdl (programmatic dependent launch) is opt-in.
+static const int kOptionDefaults[OPT_COUNT] = {1, 1, 1, 1, 0};
 static std::atomic<int> g_options[OPT_COUNT];
 static std::atomic<bool> g_options_init{false};
 

@@ -16,7 +16,7 @@ extern char g_last_error[512];
 extern std::atomic<int64_t> g_launch_count;
 
 // run-time kernel-selection switches (hallo_b200_set_option); initial value from HALLO_B200_<NAME>
-enum Option { OPT_GEMM_TEPI = 0, OPT_GEMM_1CTA, OPT_ATTN_OCC2, OPT_ATTN_POLY, OPT_ATTN_V1, OPT_XATTN_TC, OPT_TATTN_MMA, OPT_GEMM_FILL, OPT_GN_FUSED, OPT_GEMM_SPLITK, OPT_PDL, OPT_COUNT };
+enum Option { OPT_XATTN_TC = 0, OPT_TATTN_MMA, OPT_GN_FUSED, OPT_GEMM_SPLITK, OPT_PDL, OPT_COUNT };
 int option(Option o);
 
 inline int fail(int code, const char* fmt, ...) {
@@ -62,7 +62,7 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

@@ -3,9 +3,7 @@
 #include "host_common.cu"
 #include "gemm_tc.cu"
 #include "attn_tc.cu"
-#include "attn2_tc.cu"
 #include "attn_api.cu"
-#include "xattn_tc.cu"
 #include "tattn_mma.cu"
 #include "aux.cu"
 #include "peer.cu"

@@ -1,18 +1,17 @@
 // Temporal self-attention (motion_module.py:553-609) on warp-level tensor-core MMAs.
 //
 // The op is a batch of tiny attentions -- per (pixel, head): Q [Fq x d] against K, V [Fk x d], Fk <= 32 frames --
-// whose rows lie L*ld elements apart in the token matrices.  tcgen05 (M = 128 tiles, operands through
-// descriptors) has nothing to grab here, and the job is HBM-bound anyway (q/k/v read once, o written once:
-// ~57 us at level 0), so the kernel uses mma.sync m16n8k16 -- enough to take the ~5000 scalar FMA/convert
-// instructions per thread of the CUDA-core kernel (measured 230 us at level 0, instruction-bound) off the
-// critical path:
+// whose rows lie L*ld elements apart in the token matrices.  wgmma (M = 64 tiles, operands through
+// descriptors) has nothing to grab here, and the job is HBM-bound anyway (q/k/v read once, o written once), so the
+// kernel uses mma.sync m16n8k16 -- enough to take the ~5000 scalar FMA/convert instructions per thread of the
+// CUDA-core kernel off the critical path:
 //   1. the CTA copies the Q, K, V rows of PIX pixels (all frames, all heads) into shared memory with 16-byte
 //      cp.async; rows are padded so that the 8 frame-rows of an ldmatrix fall into different bank groups;
 //   2. each warp takes (pixel, head) tasks: S = Q K^T (A, B via ldmatrix), masked softmax on the accumulator
 //      fragments (quad shuffles), O = P V (P re-packed from the S fragments, V via ldmatrix.trans), O written over
 //      the task's own Q slice in shared memory;
 //   3. the CTA copies the O rows out with coalesced 16-byte stores.
-// Opt-in (option "tattn_mma") until tests/test_aux_gpu.py::test_temporal_attention has passed with it on hardware.
+// Option "tattn_mma" (default on); 0 selects the CUDA-core kernel in aux.cu.
 #include "host_common.cuh"
 #include "ptx.cuh"
 

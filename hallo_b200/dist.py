@@ -18,8 +18,8 @@ from .engine import Shard
 
 # "peer": the frame <-> pixel swap is fused into the producing kernels' stores over NVLink peer memory (the product path);
 # "nccl": the same swap as two all_to_all_single calls per motion module (A/B baseline and safe fallback).
-# "peer" is the default on evidence: tests/test_multigpu_gpu.py green on 2 x B200 (sharded vs unsharded 5.5e-5, eagerly
-# and through the captured graph, both exchanges; profiles/r2e_summary.txt) and 1.04x faster than the NCCL variant.
+# "peer" is the default: it needs no collective inside the captured graph; tests/test_multigpu_gpu.py checks both
+# exchanges against the unsharded engine.
 DEFAULT_EXCHANGE = "peer"
 
 

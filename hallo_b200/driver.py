@@ -1,5 +1,5 @@
 """Clip driver: the sliding-window loop of scripts/inference.py:262-347 over hallo_b200's pipeline (SURVEY.md 8f rows
-2-4, BASELINE.json configs[4]).
+2-4).
 
 The reference walks a clip in 16-frame windows; window t's reference stack is [source image, last n_motion frames of
 window t-1] (the source image repeated for t = 0), its audio tokens are AudioProjModel(audio_emb[16t:16t+16]), and

@@ -2,7 +2,7 @@
 
 The reference walks an nn.Module tree and issues ~2.3k library kernels per forward
 (hallo/models/unet_3d.py:510-715 and everything below it).  Here the same arithmetic is a flat,
-pre-planned sequence of hand-written sm_100a kernels (hallo_b200/csrc) over channels-last token
+pre-planned sequence of hand-written sm_90a kernels (hallo_b200/csrc) over channels-last token
 matrices, with all weights pre-packed once and all step-invariant work hoisted out of the 40-step loop:
 
   per model load : weight packing (fused QKV, interleaved GEGLU, [Cout][tap][Cin] convs, ...)

@@ -10,7 +10,7 @@ import os
 from typing import Optional
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# HALLO_B200_LIB: load another build of the same sources (tools/gemm_trace.py: the -DHB_GEMM_TRACE build)
+# HALLO_B200_LIB: load another build of the same sources
 LIB_PATH = os.environ.get("HALLO_B200_LIB") or os.path.join(_HERE, "libhallo_b200.so")
 
 HB_F16, HB_BF16 = 0, 1

@@ -1,6 +1,6 @@
 """AudioProjModel (hallo/models/audio_proj.py:40-124): wav2vec window (bz, f, 5, 12, 768) -> 32 context tokens
 of 768 per frame (SURVEY.md A10).  36 M parameters, M = 16 rows per window -- or all windows of a clip in one call
-(hallo_b200.driver, SURVEY.md 8f row 4).  Everything runs in the sm_100a kernels: three tcgen05 GEMMs with the ReLU
+(hallo_b200.driver, SURVEY.md 8f row 4).  Everything runs in the sm_90a kernels: three wgmma GEMMs with the ReLU
 fused into the epilogue (HB_EPI_RELU) and the final LayerNorm in hallo_b200_layernorm."""
 from __future__ import annotations
 

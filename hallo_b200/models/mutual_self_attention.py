@@ -1,4 +1,4 @@
-"""ReferenceAttentionControl (hallo/models/mutual_self_attention.py:39-496) for the B200 engine.
+"""ReferenceAttentionControl (hallo/models/mutual_self_attention.py:39-496) for the H100 engine.
 
 read  mode: attaches to hallo_b200's UNet3DConditionModel; update(writer) pairs the writer's banks with the 16
             spatial transformer blocks in the reference's order (stable sort by -norm1 width over module DFS order,

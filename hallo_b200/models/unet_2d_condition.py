@@ -105,7 +105,7 @@ class UNet2DConditionModel(nn.Module):
         ver = (self.device, self.dtype, tuple(p._version for p in self.parameters()))
         if self._packed is None or self._packed_version != ver:
             if self.device.type != "cuda":
-                raise RuntimeError("hallo_b200.UNet2DConditionModel runs on CUDA (sm_100a) only; there is no CPU path")
+                raise RuntimeError("hallo_b200.UNet2DConditionModel runs on CUDA (sm_90a) only; there is no CPU path")
             self._packed = ReferenceNetWeights(self.state_dict(), self.arch, self.device, self.dtype)
             self._packed_version = ver
             self._engines.clear()

@@ -1,4 +1,4 @@
-"""UNet3DConditionModel -- the reference's class surface over the sm_100a engine.
+"""UNet3DConditionModel -- the reference's class surface over the sm_90a engine.
 
 Mirrors hallo/models/unet_3d.py (UNet3DConditionModel.__init__ :121-361, .forward :510-715,
 .from_pretrained_2d :717-839): same constructor keywords, the same 1946-entry state dict (so the
@@ -209,7 +209,7 @@ class UNet3DConditionModel(nn.Module):
         ver = (self.device, self.dtype, tuple(p._version for p in self.parameters()))
         if self._packed is None or self._packed_version != ver:
             if self.device.type != "cuda":
-                raise RuntimeError("hallo_b200.UNet3DConditionModel runs on CUDA (sm_100a) only; there is no CPU path")
+                raise RuntimeError("hallo_b200.UNet3DConditionModel runs on CUDA (sm_90a) only; there is no CPU path")
             self._packed = PackedWeights(self.state_dict(), self.arch, self.device, self.dtype)
             self._packed_version = ver
             self._engines.clear()

@@ -1,4 +1,4 @@
-"""ReferenceNet on the sm_100a kernels (SURVEY.md 8f row 1): the SD-1.5 UNet2D the reference runs once per window at
+"""ReferenceNet on the sm_90a kernels (SURVEY.md 8f row 1): the SD-1.5 UNet2D the reference runs once per window at
 t = 0 on the reference image + motion frames (hallo/models/unet_2d_condition.py forward :905-1356, blocks
 unet_2d_blocks.py, transformer_2d.py:245-420, BasicTransformerBlock attention.py:79-407) whose per-block
 `norm1(hidden_states)` are the K/V banks of the denoising UNet's spatial attention (write mode,

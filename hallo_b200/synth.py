@@ -177,3 +177,10 @@ def host_threads() -> int:
     except Exception:
         pass
     return max(1, n)
+
+
+def golden_sample_index(numel: int) -> torch.Tensor:
+    """Fixed, seeded half of the element indices of a flattened output: golden vectors too large to store whole keep
+    these elements only (tests/golden, written by oracle/make_golden.py)."""
+    g = torch.Generator().manual_seed(0)
+    return torch.randperm(numel, generator=g)[: numel // 2].sort().values

@@ -1,5 +1,5 @@
 /*
- * hallo_b200 -- C ABI of the sm_100a kernels behind the Hallo denoising hot path.
+ * hallo_b200 -- C ABI of the sm_90a kernels behind the Hallo denoising hot path.
  *
  * The reference (fudan-generative-vision/hallo) has no FFI/operator layer of its own: its
  * hot path is Python classes over torch library calls (SURVEY.md section 8b).  This header is
@@ -52,14 +52,8 @@ int hallo_b200_device_error(unsigned int* code_out);
 int64_t hallo_b200_launch_count(int reset);
 /* Kernel-selection switches (A/B measurements; results are identical up to rounding whatever the setting).  Each
  * option starts from the environment variable HALLO_B200_<NAME> (upper case) or its default and can be changed at run
- * time; unknown names return HB_ERR_BAD_SHAPE / -1.  Defaults are the kernels that won their hardware A/B run.
- *   "gemm_tepi"   GEMM / conv epilogue staged through shared memory and written by TMA stores        (default 1)
- *   "gemm_1cta"   force the single-CTA GEMM kernel                                                    (default 0)
- *   "gemm_fill"   narrower GEMM N tiles (128 / 64) when the widest tile would leave SMs idle          (default 1)
- *   "attn_occ2"   head_dim 40: 64-key steps and two CTAs (four query tiles) per SM                    (default 1)
- *   "attn_poly"   n: every n-th exponential on the FMA pipe (2..4), 0 = all on the SFU               (default 0)
- *   "attn_v1"     force the single-tile attention kernel                                              (default 0)
- *   "xattn_tc"    tcgen05 cross-attention (0: CUDA-core kernel)                                       (default 1)
+ * time; unknown names return HB_ERR_BAD_SHAPE / -1.
+ *   "xattn_tc"    cross-attention on wgmma tensor cores (0: CUDA-core kernel)                        (default 1)
  *   "tattn_mma"   temporal attention on warp-level tensor-core MMAs (0: CUDA cores)                   (default 1)
  *   "gn_fused"    one-launch GroupNorm when a (frame, group) slab fits shared memory                  (default 1)
  *   "gemm_splitk" split the K loop of a GEMM / conv whose tiles fill less than half of the SMs over several CTAs
@@ -70,7 +64,7 @@ int hallo_b200_set_option(const char* name, int value);
 int hallo_b200_get_option(const char* name);
 
 /* ------------------------------------------------------------------------------------------
- * hallo_b200_gemm -- C = epilogue(A * W^T) on tcgen05 tensor cores, TMA-fed, TMEM accumulators.
+ * hallo_b200_gemm -- C = epilogue(A * W^T) on wgmma tensor cores, TMA-fed, register accumulators.
  *
  * Replaces every nn.Linear / 1x1 conv / 3x3 conv on the path:
  *   to_q/to_k/to_v/to_out           diffusers Attention used at hallo/models/attention.py:479-503,
@@ -166,14 +160,15 @@ int hallo_b200_gemm(const hb_gemm_params* p, hb_stream_t stream);
 long long hallo_b200_gemm_workspace_bytes(void);
 /* split factor the most recent hallo_b200_gemm call of this process used (1 = unsplit): tests / diagnostics */
 int hallo_b200_gemm_last_splits(void);
-/* The split-K decision itself (host arithmetic, no device needed): `tiles` output tiles (CTA pairs count as one) on
- * `sm_units` SMs (pairs: SMs / 2), reduction length K, tile width bn, the caller's workspace size and the value of option
+/* The split-K decision itself (host arithmetic, no device needed): `tiles` output tiles of 128 x bn on `sm_units` SMs
+ * (hallo_b200_gemm passes the device's SM count, cta_group 1 and bn 160), reduction length K, the caller's workspace
+ * size and the value of option
  * "gemm_splitk" (0 = off, 1 = default threshold K >= 2048, n > 1 = K >= 64 n).  Returns the split factor, 1 = unsplit. */
 int hallo_b200_gemm_choose_splits(int tiles, int sm_units, int K, int cta_group, int bn, long long workspace_bytes,
                                   int option_value);
 
 /* ------------------------------------------------------------------------------------------
- * hallo_b200_attention -- fused softmax(Q K^T / sqrt(d)) V, tcgen05 + TMEM, flash-style.
+ * hallo_b200_attention -- fused softmax(Q K^T / sqrt(d)) V on wgmma, flash-style.
  *
  * Replaces diffusers Attention/AttnProcessor2_0 SDPA at
  *   hallo/models/mutual_self_attention.py:253-286  spatial self-attention with ReferenceNet KV concat

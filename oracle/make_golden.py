@@ -1,6 +1,6 @@
-"""Generates tests/golden/* by running the UNMODIFIED reference (through oracle/compat) in THIS container.
+"""Generates tests/golden/* by running the UNMODIFIED reference (through oracle/compat) on CPU.
 
-    python oracle/make_golden.py
+    HALLO_REFERENCE_ROOT=<reference checkout> python oracle/make_golden.py
 
 Fixtures (small, committed):
   unet3d_state_dict_keys.json     key -> shape of the reference UNet3D (1946 entries)  [SURVEY.md 8b]
@@ -20,8 +20,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from hallo_b200.spec import UNetConfig  # noqa: E402
-from hallo_b200.synth import (host_threads, synth_inputs, synth_refnet_inputs, synth_state_dict,  # noqa: E402
-                              synth_state_dict_2d)
+from hallo_b200.synth import (golden_sample_index, host_threads, synth_inputs, synth_refnet_inputs,  # noqa: E402
+                              synth_state_dict, synth_state_dict_2d)
 from oracle import ref_host  # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden")
@@ -37,6 +37,37 @@ CASES = [dict(h=8, f=2, seed=42, t=999, ms=(1.0, 0.9, 1.1)),
 
 def checksum(t: torch.Tensor) -> float:
     return float(t.double().abs().sum())
+
+
+def make_crosschecks():
+    """Reference outputs the CPU tests compare with: unet_ref_h8_f3.pt (UNet3D, fp32, whole), refnet_ref_h16.pt
+    (UNet2D + write-mode control at latent 16x16: a seeded sample of the output and of every bank) and
+    process_audio_emb_37x12x8.pt (scripts/inference.py's process_audio_emb on a seeded 37 x 12 x 8 input)."""
+    cfg = UNetConfig()
+    unet = ref_host.build_reference_unet()
+    unet.load_state_dict(synth_state_dict(cfg, seed=0), strict=True)
+    c = dict(h=8, f=3, seed=7, t=123, ms=(0.7, 1.3, 1.0))
+    inp = synth_inputs(cfg, c["h"], c["h"], c["f"], seed=c["seed"], timestep=c["t"], motion_scale=c["ms"])
+    ref_host.attach_reader(unet, inp["banks"])
+    torch.save(dict(case=c, out=ref_host.run_reference_unet(unet, inp).float().clone()), os.path.join(GOLD, "unet_ref_h8_f3.pt"))
+    u2 = ref_host.build_reference_unet2d()
+    u2.load_state_dict(synth_state_dict_2d(cfg), strict=True)
+    out, banks, names = ref_host.run_reference_net(u2, synth_refnet_inputs(cfg, 16, 16, seed=11))
+    g = torch.Generator().manual_seed(0)
+
+    def sample(t, k):
+        idx = torch.randperm(t.numel(), generator=g)[:k].sort().values
+        return dict(idx=idx.int(), val=t.flatten()[idx].float().clone(), shape=list(t.shape))
+    torch.save(dict(case=dict(h=16, seed=11), out=sample(out, 32768), bank_names=names,
+                    banks={n: sample(b, 4096) for n, b in zip(names, banks)}), os.path.join(GOLD, "refnet_ref_h16.pt"))
+    import ast
+    src = open(os.path.join(ref_host.REFERENCE_ROOT, "scripts", "inference.py")).read()
+    fn = next(n for n in ast.parse(src).body if isinstance(n, ast.FunctionDef) and n.name == "process_audio_emb")
+    ns = {"torch": torch}
+    exec(compile(ast.Module(body=[fn], type_ignores=[]), "inference.py", "exec"), ns)
+    emb = torch.randn(37, 12, 8, generator=torch.Generator().manual_seed(0))
+    torch.save(dict(emb_seed=0, emb_shape=list(emb.shape), out=ns["process_audio_emb"](emb).clone()),
+               os.path.join(GOLD, "process_audio_emb_37x12x8.pt"))
 
 
 def make_refnet():
@@ -131,8 +162,15 @@ def main():
         out = ref_host.run_reference_unet(unet, inp)
         for hk in hooks:
             hk.remove()
-        # full-size outputs are stored in fp16 (rounding 5e-4 relative, far below the 1e-2 tolerance) to keep fixtures small
-        fx = dict(case=c, out=(out.clone() if out.numel() < (1 << 18) else out.half()), taps=taps, weight_checksums=wsum,
+        # full-size outputs are stored in fp16 (rounding 5e-4 relative, far below the 1e-2 tolerance) to keep fixtures small;
+        # above 2^19 elements only the seeded half golden_sample_index() picks is kept (fixtures stay under 1 MB)
+        if out.numel() < (1 << 18):
+            outs = dict(out=out.clone())
+        elif out.numel() < (1 << 19):
+            outs = dict(out=out.half())
+        else:
+            outs = dict(out_shape=list(out.shape), out_sample=out.flatten()[golden_sample_index(out.numel())].half())
+        fx = dict(case=c, **outs, taps=taps, weight_checksums=wsum,
                   input_checksums=dict(sample=checksum(inp["sample"]), audio=checksum(inp["audio_embedding"]),
                                        bank0=checksum(inp["banks"]["mid_block.attentions.0"].float())),
                   torch_version=torch.__version__)
@@ -142,6 +180,7 @@ def main():
     if only is None:
         make_refnet()
         make_audio_proj()
+        make_crosschecks()
 
 
 if __name__ == "__main__":

@@ -4,8 +4,8 @@ Self-contained plain-PyTorch restatement of the reference's denoising hot path:
   UNet3DConditionModel.forward on the SHIPPED branch (train()-mode + gradient checkpointing, SURVEY Q1)
   with ReferenceAttentionControl in read mode (CFG), + the CFG combine + DDIM v-prediction update.
 
-It exists because /root/reference and diffusers are absent on the GPU box.  It is pinned here, in
-the build container, against the unmodified reference files run through oracle/compat
+It exists because neither the reference checkout nor diffusers is a dependency of this project.  It is pinned
+against the unmodified reference files run through oracle/compat
 (tests/test_oracle_cpu.py::test_port_matches_reference_host, and the committed fixtures made by
 oracle/make_golden.py).  The reference itself ships no tests / golden vectors for this path
 (SURVEY.md section 4), so beyond that cross-check parity is "unpinned" by the upstream project.

@@ -1,9 +1,9 @@
 """ORACLE / test infrastructure -- never imported by hallo_b200/.
 
-Hosts the UNMODIFIED reference hot-path files from /root/reference on CPU through the compat
-shim in oracle/compat (diffusers==0.27.2 / xformers are absent from the image; SURVEY.md 8c).
-Only usable where /root/reference exists (this container); the GPU box uses the committed
-fixtures under tests/golden/ and the self-contained restatement in oracle/port.py.
+Hosts the UNMODIFIED reference hot-path files from a reference checkout (named by $HALLO_REFERENCE_ROOT) on CPU
+through the compat shim in oracle/compat (diffusers==0.27.2 / xformers are not dependencies; SURVEY.md 8c).
+oracle/make_golden.py uses it to write the fixtures under tests/golden/; the tests compare with those fixtures
+and with the self-contained restatement in oracle/port.py.
 """
 from __future__ import annotations
 
@@ -12,7 +12,7 @@ import sys
 
 import torch
 
-REFERENCE_ROOT = os.environ.get("HALLO_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("HALLO_REFERENCE_ROOT", "")
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
 

@@ -1,4 +1,4 @@
-"""GPU parity of hallo_b200_attention (tcgen05 flash attention with in-kernel reference-KV concat)
+"""GPU parity of hallo_b200_attention (wgmma flash attention with in-kernel reference-KV concat)
 against a plain PyTorch fp32 softmax(QK^T/sqrt d)V of the same op."""
 import pytest
 import torch

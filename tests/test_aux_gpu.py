@@ -165,7 +165,7 @@ def _sdpa(q, k, v):
 @pytest.mark.parametrize("C,nk,L", [(320, 4, 200), (1280, 4, 200), (320, 32, 200), (640, 32, 200), (1280, 32, 200),
                                     (320, 32, 1024), (320, 4, 1024), (640, 32, 64)])
 def test_cross_attention(C, nk, L):
-    """L >= 128 runs the tcgen05 kernel (csrc/xattn_tc.cu), smaller L the CUDA-core kernel."""
+    """L >= 128 runs the wgmma kernel (csrc/attn_tc.cu), smaller L the CUDA-core kernel."""
     from hallo_b200 import ops
     dev = _dev()
     H, frames, f = 8, 4, 2

@@ -1,4 +1,4 @@
-"""GPU parity of hallo_b200_gemm (tcgen05) against a plain PyTorch fp32 reference of the same op."""
+"""GPU parity of hallo_b200_gemm (wgmma) against a plain PyTorch fp32 reference of the same op."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -156,14 +156,15 @@ def _with_splitk(fn):
     return a, splits, c
 
 
-@pytest.mark.parametrize("tepi", [1, 0])
+@pytest.mark.parametrize("pdl", [1, 0])
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("M,N,K,geglu", [(256, 1280, 1280, False), (256, 1280, 5120, False), (1024, 1280, 5120, False),
                                          (200, 960, 2560, False), (256, 320, 1024, False), (8, 1280, 1280, False),
                                          (64, 640, 2048, False), (256, 5120, 1280, True), (512, 2560, 1024, True)])
-def test_gemm_split_k_option(M, N, K, geglu, dtype, tepi):
+def test_gemm_split_k_option(M, N, K, geglu, dtype, pdl):
     """Option gemm_splitk (include/hallo_b200.h): K loop of a few-tile GEMM divided over several CTAs, fp32 partials
-    reduced by split 0 in fixed order -- every kernel template, both epilogues, full epilogue (bias, residual, row scale)."""
+    reduced by split 0 in fixed order -- plain and GEGLU epilogues with bias, residual and row scale, launched with and
+    without programmatic dependent launch (option pdl: a launch may start while its predecessor drains)."""
     from hallo_b200 import lib, ops
     dev = _dev()
     g = torch.Generator(device="cpu").manual_seed(M + N + K)
@@ -176,19 +177,19 @@ def test_gemm_split_k_option(M, N, K, geglu, dtype, tepi):
     if geglu:
         w, b = ops.pack_geglu_weight(w, b)
     out = torch.empty(M, n_out, device=dev, dtype=dtype)
-    lib.set_option("gemm_tepi", tepi)
+    was_pdl = lib.get_option("pdl")
+    lib.set_option("pdl", pdl)
     try:
         got, splits, unsplit = _with_splitk(lambda: ops.gemm(a, w, out, bias=b, residual=res, row_scale=rs, geglu=geglu))
     finally:
-        lib.set_option("gemm_tepi", 1)
-    if tepi or (M <= 256 and N <= 1280):   # (the direct epilogue picks narrow tiles for small M: the larger cases fill the SMs)
-        assert splits > 1, "shape chosen to split"
+        lib.set_option("pdl", was_pdl)
+    assert splits > 1, "shape chosen to split"
     h = a.float() @ (w.float().t())
     h = h + b.float()
     if geglu:
         h = h[:, 0::2] * F.gelu(h[:, 1::2])
     ref = h * rs.float()[:, None] + res.float()
-    print(f"M{M} N{N} K{K} geglu={geglu} tepi={tepi}: S={splits}, rel L2 vs fp32 {rel_l2(got, ref):.2e}, vs unsplit {rel_l2(got, unsplit):.2e}")
+    print(f"M{M} N{N} K{K} geglu={geglu} pdl={pdl}: S={splits}, rel L2 vs fp32 {rel_l2(got, ref):.2e}, vs unsplit {rel_l2(got, unsplit):.2e}")
     assert rel_l2(got, ref) < TOL[dtype]
     assert rel_l2(got, unsplit) < TOL[dtype]
 

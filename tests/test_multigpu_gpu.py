@@ -1,4 +1,4 @@
-"""Multi-GPU parity (needs >= 2 CUDA devices; skipped on a 1-GPU box): a frame-sharded window -- frame <-> pixel
+"""Multi-GPU parity (needs >= 2 CUDA devices; skipped on a 1-GPU machine): a frame-sharded window -- frame <-> pixel
 ownership swapped around every motion module through peer memory (fused kernel stores + flag barriers) or through NCCL
 all-to-alls -- must reproduce the unsharded engine's latents.  Runs tests/mgpu_worker.py under torchrun."""
 import json

@@ -1,5 +1,5 @@
 """CPU tests of the oracle: the restatement (oracle/port.py) against the committed golden vectors made from
-the UNMODIFIED reference (oracle/make_golden.py), against the live reference when /root/reference is present,
+the UNMODIFIED reference (oracle/make_golden.py), against stored outputs of the reference run through oracle/ref_host.py,
 and against independent formulas."""
 import json
 import os
@@ -70,17 +70,14 @@ def test_port_matches_golden(cfg, sd, name):
 
 
 def test_port_matches_reference_host(cfg, sd):
-    """Live cross-check against the unmodified reference files (only where /root/reference exists)."""
-    from oracle import port, ref_host
-    if not ref_host.available():
-        pytest.skip("reference tree not present on this box")
-    unet = ref_host.build_reference_unet()
-    unet.load_state_dict(sd, strict=True)
-    inp = synth_inputs(cfg, 8, 8, 3, seed=7, timestep=123, motion_scale=(0.7, 1.3, 1.0))
-    ref_host.attach_reader(unet, inp["banks"])
-    ref = ref_host.run_reference_unet(unet, inp)
+    """The port against the unmodified reference UNet3D in fp32 (tests/golden/unet_ref_h8_f3.pt, written by running the
+    reference files through oracle/ref_host.py on the same seeded weights and inputs)."""
+    from oracle import port
+    fx = torch.load(os.path.join(GOLD, "unet_ref_h8_f3.pt"), weights_only=False)
+    c = fx["case"]
+    inp = synth_inputs(cfg, c["h"], c["h"], c["f"], seed=c["seed"], timestep=c["t"], motion_scale=c["ms"])
     out = port.unet_forward(sd, cfg, inp)
-    assert rel_l2(out, ref) < 2e-5
+    assert rel_l2(out, fx["out"]) < 2e-5
 
 
 def test_attention_restatement_vs_sdpa():
@@ -154,25 +151,28 @@ def test_refnet_port_matches_golden(cfg):
 
 
 def test_refnet_port_matches_reference_host(cfg):
-    """Live cross-check where /root/reference exists: hosted reference UNet2D + reference writer vs the port (fp32)."""
-    from oracle import port, ref_host
-    if not ref_host.available():
-        pytest.skip("reference tree not present (GPU box)")
+    """The port against the unmodified reference UNet2D + reference writer in fp32 (tests/golden/refnet_ref_h16.pt: a
+    seeded sample of the output and of every bank, written through oracle/ref_host.py on the same seeded inputs)."""
     from hallo_b200.synth import synth_refnet_inputs, synth_state_dict_2d
+    from oracle import port
+    fx = torch.load(os.path.join(GOLD, "refnet_ref_h16.pt"), weights_only=False)
     torch.set_num_threads(host_threads())
     sd2 = synth_state_dict_2d(cfg)
-    unet = ref_host.build_reference_unet2d()
-    unet.load_state_dict(sd2, strict=True)
-    inp = synth_refnet_inputs(cfg, 16, 16, seed=11)
-    out, banks, names = ref_host.run_reference_net(unet, inp)
+    inp = synth_refnet_inputs(cfg, fx["case"]["h"], fx["case"]["h"], seed=fx["case"]["seed"])
     o2, b2 = port.reference_net_forward(sd2, cfg, inp)
+    names = fx["bank_names"]
+
+    def picked(t, s):
+        assert list(t.shape) == s["shape"]
+        return t.flatten()[s["idx"].long()]
+    out = fx["out"]["val"]
     assert names == [n for n, _ in reader_bank_order(cfg)]
-    assert rel_l2(o2, out) < 2e-5
-    assert max(rel_l2(b2[n], b) for n, b in zip(names, banks)) < 2e-5
+    assert rel_l2(picked(o2, fx["out"]), out) < 2e-5
+    assert max(rel_l2(picked(b2[n], fx["banks"][n]), fx["banks"][n]["val"]) for n in names) < 2e-5
     # Q10: the image tokens are tiled over the 6 samples (n % 2), not interleaved (n // 3): a restatement with
     # repeat_interleave must NOT match
     inp_sw = dict(inp)
     wrong = inp["encoder_hidden_states"].repeat_interleave(3, dim=0)
     inp_sw["encoder_hidden_states"] = wrong
     o3, _ = port.reference_net_forward(sd2, cfg, inp_sw)
-    assert rel_l2(o3, out) > 1e-3
+    assert rel_l2(picked(o3, fx["out"]), out) > 1e-3

@@ -248,7 +248,7 @@ def test_face_animate_pipeline_call_surface(model):
 
 
 def test_audio_proj_model_matches_reference_fixture():
-    """AudioProjModel (A10) -- three tcgen05 GEMMs with fused ReLU + the LayerNorm kernel -- against the output of the
+    """AudioProjModel (A10) -- three wgmma GEMMs with fused ReLU + the LayerNorm kernel -- against the output of the
     UNMODIFIED reference class (hallo/models/audio_proj.py) on the same synth weights (tests/golden/audio_proj_f4.pt,
     made by oracle/make_golden.py)."""
     from hallo_b200.models.audio_proj import AudioProjModel

@@ -1,4 +1,4 @@
-"""End-to-end GPU parity of the denoising UNet3D forward (all sm_100a kernels, fp16) against
+"""End-to-end GPU parity of the denoising UNet3D forward (all sm_90a kernels, fp16) against
  (a) the committed golden vectors produced by the UNMODIFIED reference (oracle/make_golden.py), and
  (b) the oracle restatement run on this box's CPU (fp32) on fresh seeded inputs.
 Tolerance: relative L2 <= 1e-2 (north_star); the reference's own fp16-vs-fp32 distance is ~4e-3 (SURVEY 8c)."""
@@ -60,9 +60,16 @@ def test_unet_forward_matches_reference_golden(model, name):
     c = fx["case"]
     inp = synth_inputs(UNetConfig(), c["h"], c["h"], c["f"], seed=c["seed"], timestep=c["t"], motion_scale=c["ms"])
     out = _run(m, inp, dev)
-    err = rel_l2(out, fx["out"])
+    full_shape = tuple(out.shape)
+    if "out" in fx:
+        ref, shape = fx["out"], tuple(fx["out"].shape)
+    else:                       # fixture keeps the seeded half of the elements golden_sample_index() picks
+        from hallo_b200.synth import golden_sample_index
+        ref, shape = fx["out_sample"], tuple(fx["out_shape"])
+        out = out.flatten()[golden_sample_index(out.numel()).to(out.device)]
+    err = rel_l2(out, ref)
     print(f"{name}: rel L2 vs reference fp32 = {err:.3e}")
-    assert out.shape == fx["out"].shape and err < TOL
+    assert full_shape == shape and err < TOL
 
 
 def test_unet_forward_matches_oracle_port_32x32(model):

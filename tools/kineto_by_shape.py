@@ -3,8 +3,8 @@
 `FILE.seq` lists the kernels of one graph replay in launch order (CUPTI duration, grid, name); `FILE.ops` lists the
 hallo_b200.ops calls of one eager step in the same order.  Every op launches a known set of kernels (a GroupNorm is one
 fused launch or three; everything else one), so walking both lists in step gives the warm, in-graph time of every op
-shape -- the table DESIGN.md 4.4 quotes.
-    python tools/kineto_by_shape.py gpurun_out/r2t_kineto_n1.txt [rows]"""
+shape.
+    python tools/kineto_by_shape.py FILE [rows]"""
 import re,collections,sys
 def load(prefix):
     seq=[l.rstrip('\n') for l in open(prefix+'.seq')]
@@ -14,7 +14,7 @@ def load(prefix):
         m=re.match(r'\s*([\d.]+) us\s+grid (\[.*?\]|None)\s+(.*)',l)
         ks.append((float(m.group(1)), m.group(2), m.group(3)))
     return ks,ops
-EXP={'gemm':['gemm_tc'],'conv3x3':['gemm_tc'],'conv3x3s2':['gemm_tc'],'layernorm':['layernorm'],'attention':['attn2_tc','attn_tc'],
+EXP={'gemm':['gemm_tc'],'conv3x3':['gemm_tc'],'conv3x3s2':['gemm_tc'],'layernorm':['layernorm'],'attention':['attn_tc'],
      'cross_attention':['xattn'],'temporal_attention':['tattn'],'phase_split':['phase_split'],'upsample2x':['upsample'],
      'timestep_embed':['timestep'],'im2col_latent':['im2col'],'cfg_ddim_step':['cfg_ddim'],'groupnorm':['gn_']}
 def align(prefix):

@@ -1,7 +1,7 @@
-"""Summarise `ncu --set full` reports (read here, no GPU needed) into a JSON the docs / bench.py cite:
-   python tools/ncu_summary.py gpurun_out/r2_prof_attn.ncu-rep [...] > profiles/r2_ncu_summaries.json
+"""Summarise `ncu --set full` reports (read here, no GPU needed) into JSON:
+   python tools/ncu_summary.py REPORT.ncu-rep [...] > summary.json
 and a launch list (`--metrics gpu__time_duration.sum --csv`) into per-kernel shares:
-   python tools/ncu_summary.py --launches gpurun_out/r2_launches_one_step.csv"""
+   python tools/ncu_summary.py --launches LAUNCHES.csv"""
 import collections
 import csv
 import json

@@ -1,4 +1,4 @@
-"""Runs the L0 spatial attention (with reference-KV concat) a few times -- target of `ncu -k regex:attn2_tc`."""
+"""Runs the L0 spatial attention (with reference-KV concat) a few times -- target of `ncu -k regex:attn_tc`."""
 import os
 import sys
 

@@ -72,35 +72,6 @@ __global__ void __launch_bounds__(256) ubench_mma_sync_kernel(float* out, int it
   if (s == 123.456f) out[0] = s;
 }
 
-// tcgen05.ld 32x32b.x32 throughput (TMEM -> registers): one CTA per SM, 8 warps (two per TMEM lane quarter)
-__global__ void __launch_bounds__(256) ubench_tmem_ld_kernel(float* out, int iters) {
-  __shared__ uint32_t slot;
-  const int warp = threadIdx.x >> 5;
-  if (warp == 0) tmem_alloc<512>(&slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t base = slot + (((uint32_t)(warp & 3) * 32u) << 16);
-  uint32_t acc = 0;
-  for (int it = 0; it < iters; ++it) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      uint32_t r[32];
-      tmem_ld_x32(base + ((i * 32 + (warp >> 2) * 256) & 511), r);
-      tmem_ld_wait();
-#pragma unroll
-      for (int k = 0; k < 32; ++k) acc ^= r[k];
-    }
-  }
-  if (acc == 0x12345678u) out[0] = 1.f;
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<512>(slot);
-  }
-}
-
 }  // namespace hb
 
 // returns ops (thread-level instructions) executed per launch; caller times it
@@ -117,10 +88,6 @@ extern "C" int hb_ubench_exp(int mode, int iters, float* scratch, hb_stream_t st
     case 5: ubench_exp_kernel<5><<<grid, 256, 0, s>>>(scratch, iters, 0.5f); break;
     case 6: ubench_exp_kernel<6><<<grid, 256, 0, s>>>(scratch, iters, 0.5f); break;
     case 7: ubench_mma_sync_kernel<<<grid, 256, 0, s>>>(scratch, iters); break;
-    case 8:                                           // one CTA per SM: TMEM is allocated whole
-      ubench_tmem_ld_kernel<<<num_sms(), 256, 0, s>>>(scratch, iters);
-      HB_LAUNCH_CHECK();
-      return num_sms() * 256;
     default: return fail(HB_ERR_BAD_SHAPE, "ubench mode %d", mode);
   }
   HB_LAUNCH_CHECK();
