@@ -7,8 +7,9 @@ contracts, same RNG contract (CPU generator -> initial latents), same output obj
 
 What changed is who runs the 40-step loop (:384-427): instead of 40 x {torch.cat, UNet module walk, CFG,
 scheduler.step} this hands the window to hallo_b200.engine.DenoiseEngine, which replays one captured CUDA
-graph per step (UNet3D forward + CFG combine + DDIM update, all sm_90a kernels).  VAE, ReferenceNet,
-face_locator and image_proj are the caller's modules (outside the hot path, SURVEY.md 8f).
+graph per step (UNet3D forward + CFG combine + DDIM update, all sm_90a kernels).  The VAE's encode / decode run on
+hallo_b200.vae_engine (sm_90a kernels as well) when `vae` is an SD-1.5 AutoencoderKL on CUDA in fp16 / bf16, and
+through the module itself otherwise.  ReferenceNet, face_locator and image_proj are the caller's modules.
 """
 from __future__ import annotations
 
@@ -19,6 +20,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from .. import vae_engine
 from ..models.mutual_self_attention import ReferenceAttentionControl
 from ..scheduler import coef_table_of
 
@@ -39,6 +41,20 @@ class FaceAnimatePipeline:
         self.vae_scale_factor: int = 2 ** (len(self.vae.config.block_out_channels) - 1)
         self.use_cuda_graph = True
         self.last_timing = {}
+        self._vae_engine = None                  # (version key of self.vae, vae_engine.EngineVAE)
+
+    def _vae_call(self):
+        """What the VAE calls go through.  An nn.Module with the SD-1.5 AutoencoderKL grammar, on CUDA in fp16 or bf16,
+        runs on the library's kernels (hallo_b200.vae_engine), packed once and repacked when its parameters change;
+        anything else (another architecture, CPU, fp32) is called as it is."""
+        m = self.vae
+        if not vae_engine.runs_on_engine(m):
+            return m
+        key = vae_engine.version_key(m)
+        if self._vae_engine is None or self._vae_engine[0] != key:
+            self._vae_engine = None                                               # release the old packing first
+            self._vae_engine = (key, vae_engine.EngineVAE(m))
+        return self._vae_engine[1]
 
     # DiffusionPipeline.to(device=, dtype=) (scripts/inference.py:262)
     def to(self, device=None, dtype=None):
@@ -83,8 +99,9 @@ class FaceAnimatePipeline:
         b = latents.shape[0]
         latents = latents.permute(0, 2, 1, 3, 4).reshape(b * video_length, *latents.shape[1:2], *latents.shape[3:])
         video = []
+        vae = self._vae_call()
         for i in range(0, latents.shape[0], chunk):
-            video.append(self.vae.decode(latents[i:i + chunk].to(self.vae.dtype)).sample)
+            video.append(vae.decode(latents[i:i + chunk].to(self.vae.dtype)).sample)
         video = torch.cat(video)
         video = video.reshape(b, video_length, *video.shape[1:]).permute(0, 2, 1, 3, 4)
         video = (video / 2 + 0.5).clamp(0, 1).float()
@@ -121,7 +138,7 @@ class FaceAnimatePipeline:
                   lip=dup(pixel_values_lip_mask), src_latent=None, src_key=None)
         if source_image is not None:
             src = self._preprocess_ref(source_image, height, width).to(dtype=self.vae.dtype, device=self.vae.device)
-            st["src_latent"] = self.vae.encode(src).latent_dist.mean * 0.18215
+            st["src_latent"] = self._vae_call().encode(src).latent_dist.mean * 0.18215
         return st
 
     def _window_shard(self, video_length):
@@ -175,10 +192,10 @@ class FaceAnimatePipeline:
         ref = ref_image.reshape(-1, *ref_image.shape[2:])                       # "b f c h w -> (b f) c h w"
         if static.get("src_latent") is not None:                                # source latent hoisted: motion frames only
             mot = self._preprocess_ref(ref[1:], height, width).to(dtype=self.vae.dtype, device=self.vae.device)
-            ref_latents = torch.cat([static["src_latent"], self.vae.encode(mot).latent_dist.mean * 0.18215], dim=0)
+            ref_latents = torch.cat([static["src_latent"], self._vae_call().encode(mot).latent_dist.mean * 0.18215], dim=0)
         else:
             ref = self._preprocess_ref(ref, height, width).to(dtype=self.vae.dtype, device=self.vae.device)
-            ref_latents = self.vae.encode(ref).latent_dist.mean * 0.18215        # (1 + n_motion, 4, h, w)
+            ref_latents = self._vae_call().encode(ref).latent_dist.mean * 0.18215  # (1 + n_motion, 4, h, w)
         audio = torch.cat([torch.zeros_like(audio_tensor), audio_tensor], dim=0).to(dtype=unet.dtype, device=unet.device)
         e_b.record()
 

@@ -11,7 +11,8 @@ static int dispatch_attn(const hb_attention_params* p, cudaStream_t s) {
     case 40: return launch_attn<T, 40, 3, 2>(p, s);
     case 80: return launch_attn<T, 80, 2, 1>(p, s);
     case 160: return launch_attn<T, 160, 2, 1>(p, s);
-    default: return fail(HB_ERR_BAD_SHAPE, "attention: head_dim %d not in {40, 80, 160}", p->head_dim);
+    case 512: return launch_attn_wide<T>(p, s);     // one head, V / O columns split over 4 CTAs
+    default: return fail(HB_ERR_BAD_SHAPE, "attention: head_dim %d not in {40, 80, 160, 512}", p->head_dim);
   }
 }
 

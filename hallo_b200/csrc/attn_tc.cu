@@ -16,6 +16,8 @@
 // Cross-attention (hallo_b200_cross_attention, <= 32 image / audio keys per frame) runs the same kernel with one
 // key tile: the key frame is frame / kv_frame_div, and each mask region has its own query and key column groups.
 //
+// Head dim 512 (the VAE) has its own kernel, attn_wide_kernel, at the end of this file.
+//
 // Head dims 40 / 80 / 160 are not multiples of the 64-element swizzle span: TMA boxes of 64 columns
 // over a (d, head, token, frame) tensor map zero-fill the columns >= d, so Q/K/V stay unpadded in HBM.
 #include "host_common.cuh"
@@ -371,6 +373,263 @@ int xattn_tc_try(int dtype, const void* Q, long long ldq, int q_region_stride, c
     return dispatch_xattn<__nv_bfloat16>(dtype, Q, ldq, K, V, ldkv, O, ldo, o_region_stride, frames, L, heads, head_dim,
                                          n_keys, kv_frame_div, regions, s);
   return 1;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Head dim 512, one head: the VAE mid-block attention (diffusers Attention(heads=1, bias=True) over the (h/8)(w/8)
+// tokens of a frame).  A 64 x 512 fp32 O accumulator does not fit in a warpgroup's registers, and a 128 x 512 Q tile
+// leaves too little shared memory for a whole-row K ring.  So the V / O columns are split over kWideSplit CTAs of
+// kWideDv columns each (blockIdx.y); every CTA computes the full 512-wide Q K^T of its 128 queries (the recomputation
+// is (kWideSplit - 1) / kWideSplit of the Q K^T work, ~2 % of a VAE decode) and keeps scores and softmax in fp32.
+//
+//   shared memory: Q tile 128 x 512 (8 swizzle chunks of 64 columns, loaded once)         128 KB
+//                  K ring of kWideKStages chunks, each 64 keys x 64 columns                  64 KB
+//                  V ring of kWideVStages tiles, each 64 keys x kWideDv columns              32 KB
+//   warps 0-7: two consumer warpgroups (64 query rows each); S = sum over the 8 chunks of Q_c K_c^T, each chunk slot
+//              handed back to the producer as soon as its MMAs have retired; then the same online softmax and
+//              O += P V as attn_tc_kernel.
+//   warp 8:    TMA producer.
+constexpr int kWideD = 512;
+constexpr int kWideDv = 128;
+constexpr int kWideSplit = kWideD / kWideDv;
+constexpr int kWideBN = 64;
+constexpr int kWideKStages = 8;
+constexpr int kWideVStages = 2;
+constexpr int kWideQBytes = (kWideD / 64) * 128 * 128;
+constexpr int kWideKBytes = kWideBN * 128;                     // one 64-column chunk of a key tile
+constexpr int kWideVBytes = (kWideDv / 64) * kWideBN * 128;    // kWideDv columns of a key tile
+constexpr int kWideOffK = kWideQBytes;
+constexpr int kWideOffV = kWideOffK + kWideKStages * kWideKBytes;
+constexpr int kWideOffBar = kWideOffV + kWideVStages * kWideVBytes;
+constexpr int kWideSmem = kWideOffBar + 256 + 1024;
+static_assert(kWideSmem <= 232448, "wide attention smem budget");
+
+template <typename T>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attn_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                 const __grid_constant__ CUtensorMap tmV, const AttnDev p) {
+  constexpr int BN = kWideBN;
+  constexpr int RS = BN / 2;
+  constexpr int RO = kWideDv / 2;
+  constexpr int kChunks = kWideD / 64;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWideOffBar);
+  uint64_t* q_full = bars;
+  uint64_t* k_full = bars + 1;
+  uint64_t* k_empty = k_full + kWideKStages;
+  uint64_t* v_full = k_empty + kWideKStages;
+  uint64_t* v_empty = v_full + kWideVStages;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int qt = blockIdx.x;
+  const int vcol0 = blockIdx.y * kWideDv;
+  const int frame = blockIdx.z;
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int s = 0; s < kWideKStages; ++s) {
+      mbar_init(&k_full[s], 1);
+      mbar_init(&k_empty[s], kAttnConsumers);
+    }
+    for (int s = 0; s < kWideVStages; ++s) {
+      mbar_init(&v_full[s], 1);
+      mbar_init(&v_empty[s], kAttnConsumers);
+    }
+    fence_barrier_init();
+  }
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+  }
+  __syncthreads();
+  pdl_wait();
+  pdl_launch();
+  const int ntiles = (p.Lk + BN - 1) / BN;
+
+  if (warp == 8) {
+    // ============================ TMA producer ============================
+    if (lane == 0) {
+      mbar_arrive_expect_tx(q_full, kWideQBytes);
+#pragma unroll
+      for (int c = 0; c < kChunks; ++c) tma_load_4d(smem + c * (128 * 128), &tmQ, q_full, c * 64, 0, qt * 128, frame);
+      int ks = 0, vs = 0;
+      uint32_t kph = 0, vph = 0;
+      for (int j = 0; j < ntiles; ++j) {
+        for (int c = 0; c < kChunks; ++c) {
+          mbar_wait(&k_empty[ks], kph ^ 1, 0x61);
+          mbar_arrive_expect_tx(&k_full[ks], kWideKBytes);
+          tma_load_4d(smem + kWideOffK + ks * kWideKBytes, &tmK, &k_full[ks], c * 64, 0, j * BN, frame);
+          if (++ks == kWideKStages) {
+            ks = 0;
+            kph ^= 1;
+          }
+        }
+        mbar_wait(&v_empty[vs], vph ^ 1, 0x62);
+        mbar_arrive_expect_tx(&v_full[vs], kWideVBytes);
+#pragma unroll
+        for (int c = 0; c < kWideDv / 64; ++c)
+          tma_load_4d(smem + kWideOffV + vs * kWideVBytes + c * (BN * 128), &tmV, &v_full[vs], vcol0 + c * 64, 0,
+                      j * BN, frame);
+        if (++vs == kWideVStages) {
+          vs = 0;
+          vph ^= 1;
+        }
+      }
+    }
+    return;
+  }
+
+  // ============================ consumer warpgroups ============================
+  const int wg = threadIdx.x >> 7;
+  const int r0 = (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t sQ = smem_u32(smem) + wg * (64 * 128);
+  const uint32_t sK = smem_u32(smem + kWideOffK);
+  const uint32_t sV = smem_u32(smem + kWideOffV);
+  float o[RO];
+#pragma unroll
+  for (int i = 0; i < RO; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY};
+  float l_sum[2] = {0.f, 0.f};
+  mbar_wait(q_full, 0, 0x71);
+
+  int ks = 0, vs = 0;
+  uint32_t kph = 0, vph = 0;
+  for (int j = 0; j < ntiles; ++j) {
+    const int key0 = j * BN;
+    float s[RS];
+    int prev = -1;
+#pragma unroll 1
+    for (int c = 0; c < kChunks; ++c) {
+      mbar_wait(&k_full[ks], kph, 0x72);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        Wgmma<BN, T>::ss(s, make_desc_sw128(sQ + c * (128 * 128) + k * 32, 16, 1024),
+                         make_desc_sw128(sK + ks * kWideKBytes + k * 32, 16, 1024), (c | k) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();                       // the MMAs of chunk c - 1 have retired: its slot goes back
+      if (prev >= 0) mbar_arrive(&k_empty[prev]);
+      prev = ks;
+      if (++ks == kWideKStages) {
+        ks = 0;
+        kph ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_pin(s);
+    mbar_arrive(&k_empty[prev]);
+
+    if (key0 + BN > p.Lk) {
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (key0 + 8 * i + cq + e >= p.Lk) {
+            s[4 * i + e] = -INFINITY;
+            s[4 * i + 2 + e] = -INFINITY;
+          }
+    }
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      mx[0] = max3(mx[0], s[4 * i], s[4 * i + 1]);
+      mx[1] = max3(mx[1], s[4 * i + 2], s[4 * i + 3]);
+    }
+    float f[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float m_new = fmaxf(m_run[h], mx[h] * p.scale_log2);     // every key tile has at least one valid key
+      f[h] = fast_exp2(m_run[h] - m_new);
+      m_run[h] = m_new;
+      l_sum[h] *= f[h];
+    }
+#pragma unroll
+    for (int i = 0; i < RO / 4; ++i) {
+      o[4 * i] *= f[0];
+      o[4 * i + 1] *= f[0];
+      o[4 * i + 2] *= f[1];
+      o[4 * i + 3] *= f[1];
+    }
+    uint32_t pa[BN / 16][4];
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      const float e0 = fast_exp2(fmaf(s[4 * i], p.scale_log2, -m_run[0]));
+      const float e1 = fast_exp2(fmaf(s[4 * i + 1], p.scale_log2, -m_run[0]));
+      const float e2 = fast_exp2(fmaf(s[4 * i + 2], p.scale_log2, -m_run[1]));
+      const float e3 = fast_exp2(fmaf(s[4 * i + 3], p.scale_log2, -m_run[1]));
+      l_sum[0] += e0 + e1;
+      l_sum[1] += e2 + e3;
+      pa[i >> 1][(i & 1) * 2] = Cvt<T>::pack2(e0, e1);
+      pa[i >> 1][(i & 1) * 2 + 1] = Cvt<T>::pack2(e2, e3);
+    }
+    mbar_wait(&v_full[vs], vph, 0x73);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BN / 16; ++k)
+      Wgmma<kWideDv, T>::rs(o, pa[k], make_desc_sw128(sV + vs * kWideVBytes + k * 2048, BN * 128, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_pin(o);
+    mbar_arrive(&v_empty[vs]);
+    if (++vs == kWideVStages) {
+      vs = 0;
+      vph ^= 1;
+    }
+  }
+
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_sum[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.0f / l;
+    const int qrow = qt * 128 + wg * 64 + r0 + 8 * h;
+    if (qrow >= p.L) continue;
+    T* out = reinterpret_cast<T*>(p.O) + ((long long)frame * p.L + qrow) * p.ldo + vcol0;
+#pragma unroll
+    for (int i = 0; i < RO / 4; ++i) {
+      const int col = 8 * i + cq;
+      *reinterpret_cast<uint32_t*>(out + col) = Cvt<T>::pack2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+    }
+  }
+}
+
+// hallo_b200_attention with head_dim 512 (heads == 1, no reference keys)
+template <typename T>
+static int launch_attn_wide(const hb_attention_params* q, cudaStream_t stream) {
+  if (q->heads != 1 || q->ref_index != nullptr)
+    return fail(HB_ERR_BAD_SHAPE, "attention: head_dim 512 takes one head and no reference keys");
+  CUtensorMap tmQ, tmK, tmV;
+  int rc;
+  if ((rc = make_qkv_map(&tmQ, q->dtype, q->Q, kWideD, 1, q->L, q->frames, q->ldq, 128))) return rc;
+  if ((rc = make_qkv_map(&tmK, q->dtype, q->K, kWideD, 1, q->L, q->frames, q->ldk, kWideBN))) return rc;
+  if ((rc = make_qkv_map(&tmV, q->dtype, q->V, kWideD, 1, q->L, q->frames, q->ldv, kWideBN))) return rc;
+  AttnDev d{};
+  d.L = q->L;
+  d.Lk = q->L;
+  d.frames = q->frames;
+  d.heads = 1;
+  d.kv_frame_div = 1;
+  d.O = q->O;
+  d.ldo = q->ldo;
+  d.scale_log2 = (float)(1.4426950408889634 / sqrt((double)kWideD));
+  auto kern = attn_wide_kernel<T>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    HB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideSmem));
+    attr_set = true;
+  }
+  dim3 grid((d.L + 127) / 128, kWideSplit, d.frames);
+  HB_CUDA_CHECK(launch_kernel(kern, grid, kAttnThreads, kWideSmem, stream, tmQ, tmK, tmV, d));
+  HB_LAUNCH_CHECK();
+  return HB_OK;
 }
 
 }  // namespace hb

@@ -699,6 +699,53 @@ __global__ void im2col_latent_kernel(const float* __restrict__ lat, T* __restric
   }
 }
 
+// im2col of a small-channel fp32 NCHW image for a 3x3 stem conv, with a per-pixel affine map applied BEFORE the zero
+// padding: column (kh*3 + kw)*Cl + c of row (n, h, w) = y_c(n, h + kh - 1, w + kw - 1), y = mat (scale x) + bias, and 0
+// outside the image.  The VAE decoder's post_quant_conv (1x1, with bias) followed by the padded conv_in cannot be
+// folded into one conv exactly (the border taps would see the bias), so it is applied here, per gathered pixel.
+template <typename T>
+__global__ void im2col_affine_kernel(const float* __restrict__ x, T* __restrict__ out, int N, int Cl, int H, int W,
+                                     const float* __restrict__ mat, const float* __restrict__ bias, float scale) {
+  pdl_wait();
+  pdl_launch();
+  const long long total = (long long)N * H * W;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int w = (int)(i % W);
+  long long t = i / W;
+  const int h = (int)(t % H);
+  const int n = (int)(t / H);
+  const long long plane = (long long)H * W;
+  const float* xn = x + (long long)n * Cl * plane;
+  float v[64];
+#pragma unroll
+  for (int j = 0; j < 64; ++j) v[j] = 0.f;
+  for (int kh = 0; kh < 3; ++kh)
+    for (int kw = 0; kw < 3; ++kw) {
+      const int hh = h + kh - 1, ww = w + kw - 1;
+      if (hh < 0 || hh >= H || ww < 0 || ww >= W) continue;
+      float xin[7];
+      for (int c = 0; c < Cl; ++c) xin[c] = scale * xn[c * plane + (long long)hh * W + ww];
+      for (int c = 0; c < Cl; ++c) {
+        float y = xin[c];
+        if (mat != nullptr) {
+          y = 0.f;
+          for (int c2 = 0; c2 < Cl; ++c2) y = fmaf(mat[c * Cl + c2], xin[c2], y);
+        }
+        if (bias != nullptr) y += bias[c];
+        v[(kh * 3 + kw) * Cl + c] = y;
+      }
+    }
+  T* o = out + i * 64;
+#pragma unroll
+  for (int j = 0; j < 64; j += 8) {
+    float vv[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) vv[q] = v[j + q];
+    store8(o + j, vv);
+  }
+}
+
 // sinusoidal timestep embedding [cos | sin] (diffusers Timesteps(flip_sin_to_cos=True, shift 0)),
 // one row per CFG half; t comes from the per-step table indexed by the device step counter.
 template <typename T>
@@ -1047,6 +1094,22 @@ extern "C" int hallo_b200_im2col_latent(int dtype, const float* latents, void* o
   HB_DISPATCH_T(dtype, {
     launch_kernel(im2col_latent_kernel<T>, (int)((total + 127) / 128), 128, 0, s, 
         latents, (T*)out, batch, Cl, F, H, W, per_half_latents ? (long long)Cl * F * H * W : 0LL);
+  })
+  HB_LAUNCH_CHECK();
+  return HB_OK;
+}
+
+extern "C" int hallo_b200_im2col_affine(int dtype, const float* x, void* out, int N, int Cl, int H, int W,
+                                        const float* mat, const float* bias, float scale, hb_stream_t stream) {
+  if (!x || !out) return fail(HB_ERR_NULL, "im2col_affine: null pointer");
+  if (Cl < 1 || Cl * 9 > 64 || N < 0 || H <= 0 || W <= 0)
+    return fail(HB_ERR_BAD_SHAPE, "im2col_affine: N=%d Cl=%d H=%d W=%d", N, Cl, H, W);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const long long total = (long long)N * H * W;
+  if (total == 0) return HB_OK;
+  HB_DISPATCH_T(dtype, {
+    launch_kernel(im2col_affine_kernel<T>, (int)((total + 127) / 128), 128, 0, s, x, (T*)out, N, Cl, H, W, mat, bias,
+                  scale);
   })
   HB_LAUNCH_CHECK();
   return HB_OK;

@@ -30,6 +30,7 @@ namespace hb {
 constexpr int kBM = 128;
 constexpr int kBK = 64;
 constexpr int kBN = 160;              // divides every channel count of the UNet (320, 640, 1280, ...)
+constexpr int kBN2 = 128;             // power-of-two widths (the VAE's 128 / 256 / 512 / 1536): no wasted columns
 constexpr int kGemmStages = 6;
 constexpr int kGemmThreads = 288;     // two consumer warpgroups + the TMA warp
 constexpr int kGemmConsumers = 256;
@@ -57,7 +58,8 @@ struct GemmDev {
   float* ws;           // S > 1: fp32 partial tiles
   int* cnt;            // S > 1: arrival counters, [tile][warpgroup], zero between launches
   // conv geometry
-  int cin, img_n, img_h, img_w, box_w, box_h, box_n, tiles_w, tiles_h, stride2;
+  int cin, img_n, img_h, img_w, box_w, box_h, box_n, tiles_w, tiles_h;
+  int stride2;         // 0: stride 1, pad 1; 1: stride 2, pad 1 (conv3x3 == 2); 2: stride 2, pad (0, 1) (conv3x3 == 3)
 };
 
 // split-K: wait until `need` partial tiles have been published on *cnt, then re-arm the counter for the next launch
@@ -168,11 +170,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const int tap = kb / cin_blocks;
             const int cb = kb - tap * cin_blocks;
             const int kh = tap / 3, kw = tap - kh * 3;
-            if (p.stride2) {
+            if (p.stride2 == 1) {
               // input is stored as 4 phase planes [(p*2+q)*img_n + n][h/2][w/2][C] (x[2i+p][2j+q]);
-              // tap kh reads phase (kh==1 ? 0 : 1) at row offset (kh==0 ? -1 : 0)
+              // output o reads input rows 2o-1 .. 2o+1: tap kh reads phase (kh==1 ? 0 : 1) at row offset (kh==0 ? -1 : 0)
               const int ph = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
               tma_load_4d(sa, &tmA, &full_bar[stage], cb * kBK, w0 - (kw == 0), h0 - (kh == 0),
+                          (ph * 2 + pw) * p.img_n + n0);
+            } else if (p.stride2 == 2) {
+              // zero pad (0, 1) (diffusers Downsample2D(padding=0)): output o reads input rows 2o .. 2o+2, so tap kh
+              // reads phase (kh==1 ? 1 : 0) at row offset (kh==2 ? 1 : 0); the last row / column of the padded input
+              // lies past the plane and comes from the TMA out-of-bounds zero fill
+              const int ph = (kh == 1) ? 1 : 0, pw = (kw == 1) ? 1 : 0;
+              tma_load_4d(sa, &tmA, &full_bar[stage], cb * kBK, w0 + (kw == 2), h0 + (kh == 2),
                           (ph * 2 + pw) * p.img_n + n0);
             } else {
               tma_load_4d(sa, &tmA, &full_bar[stage], cb * kBK, w0 + kw - 1, h0 + kh - 1, n0);
@@ -457,7 +466,7 @@ static int launch_gemm(const hb_gemm_params* q, cudaStream_t stream) {
     pick_conv_box(q->img_n, q->img_h, q->img_w, &bw, &bh, &bn);
     d.cin = cin;
     d.img_n = q->img_n;
-    d.stride2 = q->conv3x3 == 2 ? 1 : 0;
+    d.stride2 = q->conv3x3 - 1;
     d.img_h = q->img_h;
     d.img_w = q->img_w;
     d.box_w = bw;
@@ -467,7 +476,7 @@ static int launch_gemm(const hb_gemm_params* q, cudaStream_t stream) {
     d.tiles_h = (q->img_h + bh - 1) / bh;
     d.tiles_m = d.tiles_w * d.tiles_h * ((q->img_n + bn - 1) / bn);
     uint64_t dims[4] = {(uint64_t)cin, (uint64_t)q->img_w, (uint64_t)q->img_h,
-                        (uint64_t)q->img_n * (q->conv3x3 == 2 ? 4 : 1)};
+                        (uint64_t)q->img_n * (q->conv3x3 >= 2 ? 4 : 1)};
     uint64_t str[3] = {(uint64_t)q->lda * 2, (uint64_t)q->lda * 2 * q->img_w,
                        (uint64_t)q->lda * 2 * q->img_w * q->img_h};
     uint32_t box[4] = {kBK, (uint32_t)bw, (uint32_t)bh, (uint32_t)bn};
@@ -526,6 +535,13 @@ static int dispatch_gemm(const hb_gemm_params* p, cudaStream_t s) {
   // anything beyond bias / group bias / row scale / residual: the epilogue with every option decided at run time
   const bool geglu = (p->flags & HB_EPI_GEGLU) != 0;
   const bool full = (p->flags & (HB_EPI_SILU | HB_EPI_RELU)) != 0 || p->ln_stats != nullptr || p->stats_out != nullptr;
+  // tile width: 160 unless N is a multiple of 128 but not of 160 (every UNet / ReferenceNet N is a multiple of 160;
+  // a 160-wide tile would leave 20-37.5 % of the MMA columns of N = 128 / 256 / 512 / 1536 empty)
+  if (p->N % kBN != 0 && p->N % kBN2 == 0) {
+    if (full) return launch_gemm<T, kBN2, kGemmStages, EPI_FULL>(p, s);
+    if (geglu) return launch_gemm<T, kBN2, kGemmStages, EPI_GEGLU>(p, s);
+    return launch_gemm<T, kBN2, kGemmStages, EPI_PLAIN>(p, s);
+  }
   if (full) return launch_gemm<T, kBN, kGemmStages, EPI_FULL>(p, s);
   if (geglu) return launch_gemm<T, kBN, kGemmStages, EPI_GEGLU>(p, s);
   return launch_gemm<T, kBN, kGemmStages, EPI_PLAIN>(p, s);
@@ -566,6 +582,8 @@ extern "C" int hallo_b200_gemm(const hb_gemm_params* p, hb_stream_t stream) {
                 HB_MAX_PEERS);
   if (p->workspace != nullptr && ((reinterpret_cast<uintptr_t>(p->workspace) & 15) != 0 || p->workspace_bytes < 0))
     return fail(HB_ERR_BAD_SHAPE, "hallo_b200_gemm: workspace must be 16-byte aligned");
+  if (p->conv3x3 < 0 || p->conv3x3 > 3)
+    return fail(HB_ERR_BAD_SHAPE, "hallo_b200_gemm: conv3x3 mode %d not in 0..3", p->conv3x3);
   if (p->A2 != nullptr && (p->K1 % kBK != 0 || p->K1 <= 0 || p->K1 >= p->K || p->conv3x3))
     return fail(HB_ERR_BAD_SHAPE, "hallo_b200_gemm: bad K split %d of %d", p->K1, p->K);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);

@@ -95,21 +95,15 @@ class PackedWeights:
         if 9 * cl > 64:
             raise NotImplementedError(f"conv_in with {cl} input channels (use_landmark=True variant) is not implemented: "
                                       "the im2col stem packs 9*in_channels <= 64 columns (Hallo ships in_channels=4)")
-        wi = torch.zeros(c0, 64, dtype=w_in.dtype, device=w_in.device)
-        wi[:, :9 * cl] = w_in.permute(0, 2, 3, 1).reshape(c0, 9 * cl)
-        put("conv_in.w", wi)
+        put("conv_in.w", ops.pack_stem_weight(w_in))
         put("conv_in.b", sd["conv_in.bias"])
         lin("time_embedding.linear_1")
         lin("time_embedding.linear_2")
         if self.kind == "3d":
             norm("conv_norm_out")
-            w_out = ops.pack_conv3x3_weight(sd["conv_out.weight"])       # [Cl, 9*C0] -> padded to 8 rows
-            wo = torch.zeros(8, w_out.shape[1], dtype=w_out.dtype, device=w_out.device)
-            wo[:w_out.shape[0]] = w_out
-            bo = torch.zeros(8, dtype=w_out.dtype, device=w_out.device)
-            bo[:w_out.shape[0]] = sd["conv_out.bias"]
-            put("conv_out.w", wo)
-            put("conv_out.b", bo)
+            # [Cl, 9*C0] -> padded to 8 rows
+            put("conv_out.w", ops.pad_rows(ops.pack_conv3x3_weight(sd["conv_out.weight"]), 8))
+            put("conv_out.b", ops.pad_rows(sd["conv_out.bias"], 8))
 
         temb_w, temb_b = [], []
         self.temb_off: Dict[str, int] = {}

@@ -5,9 +5,11 @@ hallo/animate/face_animate.py:222-246 `decode_latents` and :332-336 `vae.encode(
 is absent from this image, so this is a restatement of the published architecture (diffusers 0.27.2
 models/autoencoders/{autoencoder_kl,vae}.py, SD-1.5 config: block_out_channels (128, 256, 512, 512), 2 layers per
 block, 32 norm groups, eps 1e-6, single-head mid-block attention, latent channels 4) with diffusers' state-dict key
-names, so `sd-vae-ft-mse` checkpoints load with strict=True.  It is OUTSIDE the denoising hot path: plain PyTorch
-(cuDNN convolutions, channels_last), once per window.  Parity: unpinned against upstream (no diffusers here); the
-architecture test checks the key grammar, shapes and the encode/decode contract.
+names, so `sd-vae-ft-mse` checkpoints load with strict=True.  This module is plain PyTorch (cuDNN convolutions,
+channels_last): the CPU path, and the parity reference of hallo_b200/vae_engine.py, which runs the same state dict on
+the library's kernels -- FaceAnimatePipeline routes an SD-1.5 VAE on CUDA in fp16 / bf16 there, and calls this module
+otherwise.  Parity: unpinned against upstream (no diffusers here); the architecture test checks the key grammar,
+shapes and the encode/decode contract.
 """
 from __future__ import annotations
 

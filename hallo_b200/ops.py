@@ -91,9 +91,12 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, bias: Optional[
          group_bias: Optional[torch.Tensor] = None, rows_per_group: int = 0, alpha: float = 1.0,
          geglu: bool = False, silu: bool = False, relu: bool = False, a2: Optional[torch.Tensor] = None,
          ln_stats: Optional[torch.Tensor] = None, ln_colsum: Optional[torch.Tensor] = None, ln_eps: float = 1e-5,
-         stats_out: Optional[torch.Tensor] = None, scatter: Optional["lib.RowScatter"] = None) -> torch.Tensor:
+         stats_out: Optional[torch.Tensor] = None, scatter: Optional["lib.RowScatter"] = None,
+         split_k: bool = True) -> torch.Tensor:
     """out[M, N(/2)] = epilogue(cat([a, a2], 1) @ w.T); see include/hallo_b200.h.  With `scatter` (row_scatter()) the
-    rows go to the per-destination buffers instead of `out` (which then only supplies ldc / the shape check)."""
+    rows go to the per-destination buffers instead of `out` (which then only supplies ldc / the shape check).
+    split_k=False: no split-K workspace, so the K loop is never split and a row's result does not depend on how many
+    rows share the launch (the split is only chosen for launches whose tiles fill less than half of the SMs)."""
     p = lib.GemmParams()
     p.dtype = lib.dtype_code(a.dtype)
     M, K1 = a.shape
@@ -126,7 +129,8 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, bias: Optional[
     if scatter is not None:
         assert residual is None
         p.scatter = C.addressof(scatter)
-    _bind_workspace(p, a.device)
+    if split_k:
+        _bind_workspace(p, a.device)
     lib.check(lib.load().hallo_b200_gemm(C.byref(p), lib.current_stream()), "gemm")
     return out
 
@@ -145,8 +149,8 @@ def row_scatter(bases, seg: int, segs_per_dest: int, seg_stride: int, row0: int)
 @_timed(lambda x, w, out, **kw: f"conv3x3 n{x.shape[0]} {x.shape[1]}x{x.shape[2]} {x.shape[3]}->{w.shape[0]}")
 def conv3x3(x: torch.Tensor, w_packed: torch.Tensor, out: torch.Tensor, *, bias: Optional[torch.Tensor] = None,
             residual: Optional[torch.Tensor] = None, group_bias: Optional[torch.Tensor] = None,
-            rows_per_group: int = 0) -> torch.Tensor:
-    """x: NHWC [n, h, w, cin]; w_packed: [cout, 9*cin] ([cout][kh][kw][cin]); out: [n*h*w, cout]."""
+            rows_per_group: int = 0, split_k: bool = True) -> torch.Tensor:
+    """x: NHWC [n, h, w, cin]; w_packed: [cout, 9*cin] ([cout][kh][kw][cin]); out: [n*h*w, cout].  split_k: see gemm."""
     n, h, w_, cin = x.shape
     assert x.is_contiguous() or (x.stride(3) == 1 and x.stride(1) == w_ * x.stride(2) and x.stride(0) == h * x.stride(1))
     p = lib.GemmParams()
@@ -164,7 +168,8 @@ def conv3x3(x: torch.Tensor, w_packed: torch.Tensor, out: torch.Tensor, *, bias:
     p.alpha = 1.0
     p.conv3x3 = 1
     p.img_n, p.img_h, p.img_w = n, h, w_
-    _bind_workspace(p, x.device)
+    if split_k:
+        _bind_workspace(p, x.device)
     lib.check(lib.load().hallo_b200_gemm(C.byref(p), lib.current_stream()), "conv3x3")
     return out
 
@@ -174,6 +179,23 @@ def pack_conv3x3_weight(w: torch.Tensor) -> torch.Tensor:
     cout, cin, kh, kw = w.shape
     assert kh == 3 and kw == 3
     return w.permute(0, 2, 3, 1).reshape(cout, 9 * cin).contiguous()
+
+
+def pack_stem_weight(w: torch.Tensor) -> torch.Tensor:
+    """3x3 conv weight over a few input channels [cout, cl, 3, 3] -> [cout, 64] (k = tap*cl + c, zero columns from
+    9*cl on): the weight of the GEMM that follows im2col_latent / im2col_affine."""
+    cout, cl = w.shape[0], w.shape[1]
+    assert 9 * cl <= 64 and w.shape[2:] == (3, 3)
+    wi = torch.zeros(cout, 64, dtype=w.dtype, device=w.device)
+    wi[:, :9 * cl] = w.permute(0, 2, 3, 1).reshape(cout, 9 * cl)
+    return wi
+
+
+def pad_rows(x: torch.Tensor, rows: int) -> torch.Tensor:
+    """x [r, ...] -> [rows, ...] with zero rows appended (a narrow output head padded to the GEMM's N % 8 == 0)."""
+    out = torch.zeros((rows,) + tuple(x.shape[1:]), dtype=x.dtype, device=x.device)
+    out[:x.shape[0]] = x
+    return out
 
 
 def pack_geglu_weight(w: torch.Tensor, b: Optional[torch.Tensor]):
@@ -325,8 +347,10 @@ def phase_split(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
 
 @_timed(lambda x, w, *a, **kw: f"conv3x3s2 {x.shape[3]}->{w.shape[0]} {kw['ho']}")
 def conv3x3_stride2(x_planes: torch.Tensor, w_packed: torch.Tensor, out: torch.Tensor, *, n: int, ho: int, wo: int,
-                    bias: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """x_planes: phase planes [4*n, ho, wo, cin] from phase_split; out: [n*ho*wo, cout]."""
+                    bias: Optional[torch.Tensor] = None, pad_end: bool = False, split_k: bool = True) -> torch.Tensor:
+    """x_planes: phase planes [4*n, ho, wo, cin] from phase_split; out: [n*ho*wo, cout].
+    pad_end=False: zero padding 1 on every side (Downsample3D); True: zero padding (0, 1) on each axis, i.e. only after
+    the last row / column (diffusers Downsample2D(padding=0), the VAE encoder).  split_k: see gemm."""
     cin = x_planes.shape[-1]
     assert x_planes.is_contiguous() and x_planes.shape[0] == 4 * n
     p = lib.GemmParams()
@@ -338,9 +362,10 @@ def conv3x3_stride2(x_planes: torch.Tensor, w_packed: torch.Tensor, out: torch.T
     p.C, p.ldc = lib.ptr(out), _rowmajor_ld(out)
     p.bias = lib.ptr(bias)
     p.alpha = 1.0
-    p.conv3x3 = 2
+    p.conv3x3 = 3 if pad_end else 2
     p.img_n, p.img_h, p.img_w = n, ho, wo
-    _bind_workspace(p, x_planes.device)
+    if split_k:
+        _bind_workspace(p, x_planes.device)
     lib.check(lib.load().hallo_b200_gemm(C.byref(p), lib.current_stream()), "conv3x3_stride2")
     return out
 
@@ -355,6 +380,23 @@ def im2col_latent(latents: torch.Tensor, out: torch.Tensor, *, batch: int) -> to
                                                   C.c_void_p(lib.ptr(out)), _i(batch), _i(cl), _i(f), _i(h), _i(w),
                                                   _i(1 if (lb == batch and batch > 1) else 0),
                                                   lib.current_stream()), "im2col_latent")
+    return out
+
+
+@_timed(lambda x, out, **kw: f"im2col_affine Cl{x.shape[1]} rows{out.shape[0]}")
+def im2col_affine(x: torch.Tensor, out: torch.Tensor, *, mat: Optional[torch.Tensor] = None,
+                  bias: Optional[torch.Tensor] = None, scale: float = 1.0) -> torch.Tensor:
+    """x: fp32 NCHW [n, cl, h, w] contiguous, 9*cl <= 64; out: [n*h*w, 64].  Column (kh*3 + kw)*cl + c of row (n, y, x)
+    holds (mat @ (scale * pixel) + bias)[c] of pixel (y + kh - 1, x + kw - 1), 0 outside the image.  mat: fp32 [cl, cl]
+    or None (identity); bias: fp32 [cl] or None."""
+    n, cl, h, w = x.shape
+    assert x.dtype == torch.float32 and x.is_contiguous() and out.is_contiguous() and out.shape == (n * h * w, 64)
+    for t, shape in ((mat, (cl, cl)), (bias, (cl,))):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == shape)
+    lib.check(lib.load().hallo_b200_im2col_affine(_i(lib.dtype_code(out.dtype)), C.c_void_p(lib.ptr(x)),
+                                                  C.c_void_p(lib.ptr(out)), _i(n), _i(cl), _i(h), _i(w),
+                                                  C.c_void_p(lib.ptr(mat)), C.c_void_p(lib.ptr(bias)),
+                                                  C.c_float(scale), lib.current_stream()), "im2col_affine")
     return out
 
 

@@ -84,6 +84,10 @@ int hallo_b200_get_option(const char* name);
  *   conv3x3 == 2: stride-2 conv (Downsample3D, resnet.py:232-252).  A holds the 4 phase planes
  *        written by hallo_b200_phase_split: [4*img_n, img_h, img_w, Cin] where img_h/img_w are
  *        the OUTPUT height/width; M = img_n*img_h*img_w.
+ *   conv3x3 == 3: stride-2 conv with zero padding (0, 1) on each axis -- diffusers Downsample2D(padding=0), the VAE
+ *        encoder's downsampler: output o reads input rows 2o, 2o+1, 2o+2 (conv3x3 == 2 reads 2o-1 .. 2o+1).  Same
+ *        phase-plane input and img_h / img_w (OUTPUT size) as conv3x3 == 2; the input height / width are 2 img_h /
+ *        2 img_w, and the bottom / right pad comes from the TMA out-of-bounds fill.
  *        A conv takes bias / group_bias / row_scale / residual only (no activation, GEGLU, LayerNorm fold, stats_out).
  *   epilogue, in this order (each optional):
  *        v  = acc + bias[col] + group_bias[row / rows_per_group][col]
@@ -91,6 +95,8 @@ int hallo_b200_get_option(const char* name);
  *                                                 output has N/2 columns)
  *        v  = v * row_scale[row] * alpha + residual[row][col]
  *   Constraints: K % 64 == 0 (K1 % 64 == 0, Cin % 64 == 0); lda/ldw/ldc/ldr % 8 == 0.
+ *   Tile: 128 x 160 output tiles, or 128 x 128 when N is a multiple of 128 but not of 160 (N = 128, 256, 512, 1536 ...:
+ *        a 160-wide tile would leave up to 37.5 % of its MMA columns empty).  Chosen from N alone; no option.
  * ---------------------------------------------------------------------------------------- */
 enum hb_epi_flags {
   HB_EPI_GEGLU = 1,
@@ -161,7 +167,7 @@ long long hallo_b200_gemm_workspace_bytes(void);
 /* split factor the most recent hallo_b200_gemm call of this process used (1 = unsplit): tests / diagnostics */
 int hallo_b200_gemm_last_splits(void);
 /* The split-K decision itself (host arithmetic, no device needed): `tiles` output tiles of 128 x bn on `sm_units` SMs
- * (hallo_b200_gemm passes the device's SM count, cta_group 1 and bn 160), reduction length K, the caller's workspace
+ * (hallo_b200_gemm passes the device's SM count, cta_group 1 and the tile width it picked, 160 or 128), reduction length K, the caller's workspace
  * size and the value of option
  * "gemm_splitk" (0 = off, 1 = default threshold K >= 2048, n > 1 = K >= 64 n).  Returns the split factor, 1 = unsplit. */
 int hallo_b200_gemm_choose_splits(int tiles, int sm_units, int K, int cta_group, int bn, long long workspace_bytes,
@@ -183,7 +189,10 @@ int hallo_b200_gemm_choose_splits(int tiles, int sm_units, int K, int cta_group,
  *             (the reference tiles CFG halves over the batch: ref_index[n] = n % 2 for cond
  *             frames, -1 for uncond frames -- SURVEY quirk Q9).  NULL = plain self-attention.
  *   O       : [frames*L, ldo], same head layout.
- *   head_dim in {40, 80, 160}; scale = head_dim^-0.5; no mask, no dropout.
+ *   head_dim in {40, 80, 160, 512}; scale = head_dim^-0.5; no mask, no dropout.  Scores and softmax in fp32.
+ *   head_dim 512 (the VAE mid-block attention, diffusers Attention(heads=1) over the (h/8)(w/8) tokens of a frame):
+ *             heads == 1 and no reference keys; L may be any length.  The V / O columns are split over 4 CTAs of
+ *             128 columns, each of which recomputes the 512-wide Q K^T.
  * ---------------------------------------------------------------------------------------- */
 typedef struct {
   int32_t dtype;
@@ -251,6 +260,14 @@ int hallo_b200_phase_split(int dtype, const void* x, void* out, int N, int H, in
  * [batch, Cl, F, H, W]. */
 int hallo_b200_im2col_latent(int dtype, const float* latents, void* out, int batch, int Cl, int F, int H,
                              int W, int per_half_latents, hb_stream_t stream);
+/* im2col for a 3x3 stem conv over a small-channel fp32 NCHW image x [N, Cl, H, W] (9 Cl <= 64): out [N*H*W, 64],
+ * column (kh*3 + kw)*Cl + c of row (n, h, w) = y_c at pixel (h + kh - 1, w + kw - 1), 0 outside the image (columns
+ * >= 9 Cl are 0), where y = mat (scale x) + bias per pixel.  mat: fp32 [Cl, Cl] row-major or NULL (identity); bias:
+ * fp32 [Cl] or NULL (0).  The affine map is applied before the zero padding: the VAE decoder's post_quant_conv (1x1
+ * with bias) in front of its padded conv_in, which no folded weight reproduces at the border; with mat = bias = NULL
+ * it is the plain im2col of the encoder's RGB conv_in. */
+int hallo_b200_im2col_affine(int dtype, const float* x, void* out, int N, int Cl, int H, int W, const float* mat,
+                             const float* bias, float scale, hb_stream_t stream);
 /* diffusers Timesteps(dim, flip_sin_to_cos=True, shift 0) for t = t_table[*step] (unet_3d.py:565-587). */
 int hallo_b200_timestep_embed(int dtype, const float* t_table, const int32_t* step, void* out, int rows,
                               int dim, hb_stream_t stream);
