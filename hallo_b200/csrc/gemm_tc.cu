@@ -1,13 +1,22 @@
 // hallo_b200_gemm: persistent warp-specialised wgmma GEMM / implicit-GEMM conv3x3 (sm_90a).
 //
 //   warps 0-3, 4-7 : two consumer warpgroups.  Warpgroup g owns rows [64g, 64g + 64) of the 128 x BN tile: one
-//                    wgmma m64nBNk16 per 16-wide K step (fp32 accumulators in registers), then the epilogue
-//                    (bias / temb / GEGLU / LayerNorm fold / mask / residual / row statistics) straight from the
-//                    accumulator registers to global memory.
-//   warp 8         : TMA producer (A tile 128x64, W tile BNx64 per stage, 128B-swizzled), one elected lane.
+//                    wgmma m64nBNk16 per 16-wide K step (fp32 accumulators in registers), then the epilogue.
+//   warp 8         : TMA producer (A tile 128x64, W tile BNx64 per stage, 128B-swizzled; the residual tile), one
+//                    elected lane.
 //
 // Each warpgroup keeps one wgmma group in flight: the stage of K step i is handed back to the producer once the
 // MMAs of step i + 1 have been issued and those of step i have completed.
+//
+// Staged epilogue (bias / group bias / row scale / GEGLU / residual): every warpgroup owns a 64 x BN staging tile in
+// shared memory, stored as CW-column chunks (CW = 32 or 16, swizzled over CW * 2 bytes, so the accumulator-layout
+// accesses are free of bank conflicts).  The producer loads the tile's residual into it with TMA during the K loop;
+// the warpgroup adds the epilogue terms in place and one thread stores the chunks with TMA, whose clipping at the
+// tensor bounds replaces the M-tail and overhanging-conv-box masks.  The warpgroup then goes straight on to the next
+// tile: its store drains while that tile's MMAs run, and the staging tile is handed back to the producer (barrier
+// stg_free) after the first k-block of the next tile, once the store has read it.
+// Row scatter to peer buffers, the EPI_FULL options (activation, LayerNorm fold, row statistics) and output or
+// residual pointers that are not 16-byte aligned keep the register epilogue, which stores straight to global memory.
 //
 // Split-K (p.splits = S > 1, chosen by the host when the tiles cover less than half of the SMs): the grid holds one
 // CTA per (tile, split); split s runs k-blocks [s*kper, (s+1)*kper).  Splits 1.. store their raw fp32 accumulators to
@@ -31,7 +40,8 @@ constexpr int kBM = 128;
 constexpr int kBK = 64;
 constexpr int kBN = 160;              // divides every channel count of the UNet (320, 640, 1280, ...)
 constexpr int kBN2 = 128;             // power-of-two widths (the VAE's 128 / 256 / 512 / 1536): no wasted columns
-constexpr int kGemmStages = 6;
+constexpr int kGemmStages = 5;        // BN = 160: 5 x 36 KB of operand stages + 40 KB of staging tiles
+constexpr int kGemmStages2 = 6;       // BN = 128: 6 x 32 KB + 32 KB
 constexpr int kGemmThreads = 288;     // two consumer warpgroups + the TMA warp
 constexpr int kGemmConsumers = 256;
 
@@ -60,6 +70,8 @@ struct GemmDev {
   // conv geometry
   int cin, img_n, img_h, img_w, box_w, box_h, box_n, tiles_w, tiles_h;
   int stride2;         // 0: stride 1, pad 1; 1: stride 2, pad 1 (conv3x3 == 2); 2: stride 2, pad (0, 1) (conv3x3 == 3)
+  int staged;          // epilogue through the staging tiles and TMA stores (tmC; tmR when residual != nullptr)
+  int wg_dw, wg_dh, wg_dn;   // conv: origin of warpgroup 1's half box within the tile's box
 };
 
 // split-K: wait until `need` partial tiles have been published on *cnt, then re-arm the counter for the next launch
@@ -83,9 +95,28 @@ struct GemmSmem {
   static constexpr int kABytes = kBM * kBK * 2;
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kBarOffset = STAGES * kStageBytes;
+  static constexpr int kStgOffset = STAGES * kStageBytes;
+  static constexpr int kStgBytes = 64 * BN * 2;            // one warpgroup's staging tile
+  static constexpr int kBarOffset = kStgOffset + 2 * kStgBytes;
   static constexpr int kTotal = kBarOffset + 256 + 1024;  // + barriers + alignment slack
-  static_assert(kStageBytes % 1024 == 0, "stage alignment");
+  static_assert(kStageBytes % 1024 == 0 && kStgBytes % 1024 == 0, "stage alignment");
+  static_assert(2 * STAGES * 8 + 4 * 8 <= 256, "barrier space");
+};
+
+// Staging-tile geometry of an epilogue that writes NOUT columns per tile: CW-column chunks of 64 rows, swizzled over
+// the chunk's row width (Swizzle<log2(CW * 2 / 16), 4, 3>, what the tensor map's CU_TENSOR_MAP_SWIZZLE_{64,32}B does).
+template <int NOUT>
+struct Staging {
+  static constexpr int kCW = NOUT % 32 == 0 ? 32 : 16;
+  static constexpr int kChunks = NOUT / kCW;
+  static constexpr int kChunkBytes = 64 * kCW * 2;
+  static constexpr int kSwizzle = kCW * 2;
+  static_assert(NOUT % 16 == 0, "staging width");
+  // byte offset of element (r, c) of the 64 x NOUT tile
+  __device__ static __forceinline__ uint32_t offset(int r, int c) {
+    const uint32_t o = (uint32_t)((c / kCW) * kChunkBytes + r * (kCW * 2) + (c % kCW) * 2);
+    return o ^ (((o >> 7) & (kSwizzle / 16 - 1)) << 4);
+  }
 };
 
 // EPI fixes the epilogue at compile time: EPI_PLAIN = bias / group bias / row scale / residual, EPI_GEGLU = the same
@@ -96,24 +127,35 @@ enum { EPI_PLAIN = 0, EPI_GEGLU = 1, EPI_FULL = 2 };
 template <typename T, int BN, int STAGES, bool CONV, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-               const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
+               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
+               const __grid_constant__ CUtensorMap tmR, const GemmDev p) {
   using SM = GemmSmem<BN, STAGES>;
   static_assert(BN % 16 == 0 && BN <= 256, "BN");
   constexpr int R = BN / 2;             // accumulator registers per consumer thread
+  constexpr int NOUT = EPI == EPI_GEGLU ? BN / 2 : BN;   // output columns per tile (staged epilogue)
+  using STG = Staging<NOUT>;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* res_full = empty_bar + STAGES;   // [warpgroup]: residual tile landed in the staging tile
+  uint64_t* stg_free = res_full + 2;         // [warpgroup]: the previous tile's store has read the staging tile
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const bool staged = EPI != EPI_FULL && p.staged != 0;
+  const bool stage_resid = staged && p.residual != nullptr;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], kGemmConsumers);
+    }
+    for (int g = 0; g < 2; ++g) {
+      mbar_init(&res_full[g], 1);
+      mbar_init(&stg_free[g], 1);
     }
     fence_barrier_init();
   }
@@ -121,6 +163,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (p.K1 < p.K) tma_prefetch_desc(&tmA2);
+    if (staged) tma_prefetch_desc(&tmC);
+    if (stage_resid) tma_prefetch_desc(&tmR);
   }
   __syncthreads();
   pdl_wait();        // everything above (barriers, tensor-map prefetch) may overlap the predecessor's tail
@@ -152,13 +196,33 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       w0 = (rem - hb_ * p.tiles_w) * p.box_w;
     }
   };
+  // staging tile of warpgroup g <-> global memory (output through tmC, residual through tmR): chunk ch of the tile
+  auto stg_copy = [&](bool store, int g, int ch, int tm, int tn, int n0, int h0, int w0) {
+    uint8_t* st = smem + SM::kStgOffset + g * SM::kStgBytes + ch * STG::kChunkBytes;
+    const int c = tn * NOUT + ch * STG::kCW;
+    if (CONV) {
+      const int cw = w0 + g * p.wg_dw, chh = h0 + g * p.wg_dh, cn = n0 + g * p.wg_dn;
+      if (store) tma_store_4d(&tmC, st, c, cw, chh, cn);
+      else tma_load_4d(st, &tmR, &res_full[g], c, cw, chh, cn);
+    } else {
+      if (store) tma_store_2d(&tmC, st, c, tm * kBM + 64 * g);
+      else tma_load_2d(st, &tmR, &res_full[g], c, tm * kBM + 64 * g);
+    }
+  };
+  // chunks of tile column tn that hold output columns (N = 8 heads: one of five)
+  auto live_chunks = [&](int tn) {
+    const int left = ((EPI == EPI_GEGLU) ? p.N / 2 : p.N) - tn * NOUT;
+    const int n = (left + STG::kCW - 1) / STG::kCW;
+    return n < STG::kChunks ? n : STG::kChunks;
+  };
 
   if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = first; t < num_tiles; t += stride) {
+      int it = 0;
+      for (int t = first; t < num_tiles; t += stride, ++it) {
         int tm, tn, n0, h0, w0;
         tile_origin(t, tm, tn, n0, h0, w0);
         for (int kb = kb0; kb < kb1; ++kb) {
@@ -197,6 +261,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             phase ^= 1;
           }
         }
+        // the tile's residual, once each warpgroup's store of the previous tile has left its staging tile
+        if (stage_resid && split == 0) {
+          for (int g = 0; g < 2; ++g) {
+            if (it > 0) mbar_wait(&stg_free[g], (it - 1) & 1, 0x13);
+            const int nch = live_chunks(tn);
+            mbar_arrive_expect_tx(&res_full[g], nch * STG::kChunkBytes);
+            for (int ch = 0; ch < nch; ++ch) stg_copy(false, g, ch, tm, tn, n0, h0, w0);
+          }
+        }
       }
     }
     return;
@@ -215,10 +288,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const bool geglu = (EPI == EPI_GEGLU) || (EPI == EPI_FULL && (p.flags & HB_EPI_GEGLU) != 0);
   const int n_out = geglu ? (p.N >> 1) : p.N;
 
+  const bool stg_leader = (ct & 127) == 0;                // issues this warpgroup's TMA stores
   int stage = 0;
   uint32_t phase = 0;
   float acc[R];
-  for (int t = first; t < num_tiles; t += stride) {
+  int it = 0;
+  for (int t = first; t < num_tiles; t += stride, ++it) {
     int tm, tn, n0, h0, w0;
     tile_origin(t, tm, tn, n0, h0, w0);
     int prev = -1;
@@ -232,6 +307,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
       for (int k = 0; k < kBK / 16; ++k) Wgmma<BN, T>::ss(acc, adesc + 2 * k, bdesc + 2 * k, ((kb - kb0) | k) != 0);
       wgmma_commit();
+      // the previous tile's store has had the first k-block's MMAs to read the staging tile: hand it back
+      if (staged && it > 0 && kb == kb0 && stg_leader) {
+        bulk_wait_group_read<0>();
+        mbar_arrive(&stg_free[wg]);
+      }
       wgmma_wait<1>();
       if (prev >= 0) mbar_arrive(&empty_bar[prev]);
       prev = stage;
@@ -264,6 +344,78 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
         for (int j = 0; j < R; ++j) acc[j] += __ldcg(w + j * kGemmConsumers);
       }
+    }
+
+    if (staged) {
+      // ===================== staged epilogue: registers -> staging tile (+ residual) -> TMA store =====================
+      if (stage_resid) mbar_wait(&res_full[wg], it & 1, 0x23);
+      else if (it > 0) mbar_wait(&stg_free[wg], (it - 1) & 1, 0x24);
+      uint8_t* stg = smem + SM::kStgOffset + wg * SM::kStgBytes;
+      const int rl0 = r0 - 64 * wg;                       // rows rl0, rl0 + 8 of the warpgroup's 64-row half
+      float rs[2];
+      const T* gb_row[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r_in_tile = r0 + 8 * h;
+        long long row;
+        bool row_ok;
+        if (CONV) {
+          const int dn = r_in_tile / (p.box_h * p.box_w);
+          const int r2 = r_in_tile - dn * (p.box_h * p.box_w);
+          const int dh = r2 / p.box_w;
+          const int dw = r2 - dh * p.box_w;
+          const int in_ = n0 + dn, ih = h0 + dh, iw = w0 + dw;
+          row = ((long long)in_ * p.img_h + ih) * p.img_w + iw;
+          row_ok = in_ < p.img_n && ih < p.img_h && iw < p.img_w;
+        } else {
+          row = (long long)tm * kBM + r_in_tile;
+          row_ok = row < p.M;
+        }
+        // rows outside the output are computed from zero-filled operands and clipped by the store
+        rs[h] = p.alpha;
+        if (rscale != nullptr && row_ok) rs[h] *= Cvt<T>::to_f(rscale[row]);
+        gb_row[h] = (gbias != nullptr && row_ok) ? gbias + (row / p.rows_per_group) * p.ld_group_bias : nullptr;
+      }
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        const int col = tn * BN + 8 * i + cq;
+        if (col >= p.N) continue;
+        float2 b2 = make_float2(0.f, 0.f);
+        if (bias != nullptr) b2 = Cvt<T>::unpack2(*reinterpret_cast<const uint32_t*>(bias + col));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+          v0 += b2.x;
+          v1 += b2.y;
+          if (gb_row[h] != nullptr) {
+            const float2 g2 = Cvt<T>::unpack2(*reinterpret_cast<const uint32_t*>(gb_row[h] + col));
+            v0 += g2.x;
+            v1 += g2.y;
+          }
+          if (geglu) {
+            T* s = reinterpret_cast<T*>(stg + STG::offset(rl0 + 8 * h, 4 * i + (cq >> 1)));
+            float o = v0 * gelu_fast(v1) * rs[h];
+            if (resid != nullptr) o += Cvt<T>::to_f(*s);
+            *s = Cvt<T>::from_f(o);
+          } else {
+            uint32_t* s = reinterpret_cast<uint32_t*>(stg + STG::offset(rl0 + 8 * h, 8 * i + cq));
+            float w0_ = v0 * rs[h], w1_ = v1 * rs[h];
+            if (resid != nullptr) {
+              const float2 r2 = Cvt<T>::unpack2(*s);
+              w0_ += r2.x;
+              w1_ += r2.y;
+            }
+            *s = Cvt<T>::pack2(w0_, w1_);
+          }
+        }
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1 + wg, 128);
+      if (stg_leader) {
+        for (int ch = 0; ch < live_chunks(tn); ++ch) stg_copy(true, wg, ch, tm, tn, n0, h0, w0);
+        bulk_commit_group();
+      }
+      continue;
     }
 
     // ===================== epilogue: this thread's two rows, BN/4 columns each =====================
@@ -380,6 +532,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
   }
+  if (staged && stg_leader) bulk_wait_group<0>();   // the staging tiles must outlive the last stores
 }
 
 constexpr long long kSplitKCounterBytes = 8192;     // head of the split-K workspace: arrival counters
@@ -497,6 +650,38 @@ static int launch_gemm(const hb_gemm_params* q, cudaStream_t stream) {
     }
   }
 
+  // staged epilogue: output / residual maps with the box of one warpgroup's half tile, CW columns wide
+  constexpr int NOUT = EPI == EPI_GEGLU ? BN / 2 : BN;
+  using STG = Staging<NOUT>;
+  auto aligned16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+  d.staged = EPI != EPI_FULL && q->scatter == nullptr && aligned16(q->C) &&
+             (q->residual == nullptr || aligned16(q->residual));
+  CUtensorMap tmC = tmA, tmR = tmA;
+  if (d.staged) {
+    const uint64_t n_out = (EPI == EPI_GEGLU) ? q->N / 2 : q->N;
+    auto make_out_map = [&](CUtensorMap* m, const void* base, long long ld) {
+      if (q->conv3x3) {
+        // half box: split the tile's (w, h, n) box along its outermost dimension that is larger than 1
+        const int hn = d.box_n > 1 ? d.box_n / 2 : 1;
+        const int hh = d.box_n > 1 ? d.box_h : (d.box_h > 1 ? d.box_h / 2 : 1);
+        const int hw = d.box_n > 1 || d.box_h > 1 ? d.box_w : d.box_w / 2;
+        d.wg_dn = d.box_n > 1 ? hn : 0;
+        d.wg_dh = d.box_n == 1 && d.box_h > 1 ? hh : 0;
+        d.wg_dw = d.box_n == 1 && d.box_h == 1 ? hw : 0;
+        uint64_t dims[4] = {n_out, (uint64_t)q->img_w, (uint64_t)q->img_h, (uint64_t)q->img_n};
+        uint64_t str[3] = {(uint64_t)ld * 2, (uint64_t)ld * 2 * q->img_w, (uint64_t)ld * 2 * q->img_w * q->img_h};
+        uint32_t box[4] = {(uint32_t)STG::kCW, (uint32_t)hw, (uint32_t)hh, (uint32_t)hn};
+        return make_tmap_16b(m, q->dtype, base, 4, dims, str, box, STG::kSwizzle);
+      }
+      uint64_t dims[2] = {n_out, (uint64_t)q->M};
+      uint64_t str[1] = {(uint64_t)ld * 2};
+      uint32_t box[2] = {(uint32_t)STG::kCW, 64};
+      return make_tmap_16b(m, q->dtype, base, 2, dims, str, box, STG::kSwizzle);
+    };
+    if ((rc = make_out_map(&tmC, q->C, q->ldc)) != HB_OK) return rc;
+    if (q->residual != nullptr && (rc = make_out_map(&tmR, q->residual, q->ldr)) != HB_OK) return rc;
+  }
+
   const int tiles = d.tiles_m * d.tiles_n;
   if (tiles <= 0) return HB_OK;
   const int max_ctas = num_sms();
@@ -525,7 +710,7 @@ static int launch_gemm(const hb_gemm_params* q, cudaStream_t stream) {
     HB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal));
     attr_set[q->conv3x3 ? 1 : 0] = true;
   }
-  HB_CUDA_CHECK(launch_kernel(kern, dim3(grid), dim3(kGemmThreads), SM::kTotal, stream, tmA, tmA2, tmB, d));
+  HB_CUDA_CHECK(launch_kernel(kern, dim3(grid), dim3(kGemmThreads), SM::kTotal, stream, tmA, tmA2, tmB, tmC, tmR, d));
   HB_LAUNCH_CHECK();
   return HB_OK;
 }
@@ -538,9 +723,9 @@ static int dispatch_gemm(const hb_gemm_params* p, cudaStream_t s) {
   // tile width: 160 unless N is a multiple of 128 but not of 160 (every UNet / ReferenceNet N is a multiple of 160;
   // a 160-wide tile would leave 20-37.5 % of the MMA columns of N = 128 / 256 / 512 / 1536 empty)
   if (p->N % kBN != 0 && p->N % kBN2 == 0) {
-    if (full) return launch_gemm<T, kBN2, kGemmStages, EPI_FULL>(p, s);
-    if (geglu) return launch_gemm<T, kBN2, kGemmStages, EPI_GEGLU>(p, s);
-    return launch_gemm<T, kBN2, kGemmStages, EPI_PLAIN>(p, s);
+    if (full) return launch_gemm<T, kBN2, kGemmStages2, EPI_FULL>(p, s);
+    if (geglu) return launch_gemm<T, kBN2, kGemmStages2, EPI_GEGLU>(p, s);
+    return launch_gemm<T, kBN2, kGemmStages2, EPI_PLAIN>(p, s);
   }
   if (full) return launch_gemm<T, kBN, kGemmStages, EPI_FULL>(p, s);
   if (geglu) return launch_gemm<T, kBN, kGemmStages, EPI_GEGLU>(p, s);

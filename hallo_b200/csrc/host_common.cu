@@ -82,12 +82,15 @@ int make_tmap_16b(CUtensorMap* out, int dtype, const void* base, int rank, const
   }
   CUtensorMapDataType dt =
       dtype == HB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  if (swizzle_bytes != 128 && swizzle_bytes != 64) return fail(HB_ERR_BAD_SHAPE, "tmap swizzle %d", swizzle_bytes);
+  if (swizzle_bytes != 128 && swizzle_bytes != 64 && swizzle_bytes != 32)
+    return fail(HB_ERR_BAD_SHAPE, "tmap swizzle %d", swizzle_bytes);
   if ((uint64_t)box[0] * 2 > (uint64_t)swizzle_bytes)
     return fail(HB_ERR_BAD_SHAPE, "tmap inner box %u x 2 B exceeds the %d B swizzle span", box[0], swizzle_bytes);
   CUresult r = enc(out, dt, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   swizzle_bytes == 32   ? CU_TENSOR_MAP_SWIZZLE_32B
+                   : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                         : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     return fail(HB_ERR_CUDA,

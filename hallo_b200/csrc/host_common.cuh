@@ -51,7 +51,7 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 
 PFN_encodeTiled get_encode_tiled();
 
-// rank-R tiled tensor map over 16-bit elements, 128B swizzle, zero OOB fill.
+// rank-R tiled tensor map over 16-bit elements, 128B (or 64B / 32B) swizzle, zero OOB fill.
 // dims/strides innermost first; strides_bytes has rank-1 entries (dims 1..R-1).
 int make_tmap_16b(CUtensorMap* out, int dtype, const void* base, int rank, const uint64_t* dims,
                   const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128);

@@ -15,7 +15,7 @@ def load(prefix):
         ks.append((float(m.group(1)), m.group(2), m.group(3)))
     return ks,ops
 EXP={'gemm':['gemm_tc'],'conv3x3':['gemm_tc'],'conv3x3s2':['gemm_tc'],'layernorm':['layernorm'],'attention':['attn_tc'],
-     'cross_attention':['xattn'],'temporal_attention':['tattn'],'phase_split':['phase_split'],'upsample2x':['upsample'],
+     'cross_attention':['xattn','attn_tc'],'temporal_attention':['tattn'],'phase_split':['phase_split'],'upsample2x':['upsample'],
      'timestep_embed':['timestep'],'im2col_latent':['im2col'],'cfg_ddim_step':['cfg_ddim'],'groupnorm':['gn_']}
 def align(prefix):
     ks,ops=load(prefix)
