@@ -7,7 +7,7 @@ contracts, same RNG contract (CPU generator -> initial latents), same output obj
 
 What changed is who runs the 40-step loop (:384-427): instead of 40 x {torch.cat, UNet module walk, CFG,
 scheduler.step} this hands the window to hallo_b200.engine.DenoiseEngine, which replays one captured CUDA
-graph per step (UNet3D forward + CFG combine + DDIM update, all sm_90a kernels).  The VAE's encode / decode run on
+graph per step (UNet3D forward + CFG combine + DDIM or DPM-Solver++ update, all sm_90a kernels).  The VAE's encode / decode run on
 hallo_b200.vae_engine (sm_90a kernels as well) when `vae` is an SD-1.5 AutoencoderKL on CUDA in fp16 / bf16, and
 through the module itself otherwise.  ReferenceNet, face_locator and image_proj are the caller's modules.
 """
@@ -22,7 +22,7 @@ import torch.nn.functional as F
 
 from .. import vae_engine
 from ..models.mutual_self_attention import ReferenceAttentionControl
-from ..scheduler import coef_table_of
+from ..scheduler import sampler_table_of
 
 
 @dataclass
@@ -211,7 +211,8 @@ class FaceAnimatePipeline:
         eng.begin_window(encoder_hidden_states=ehs, audio_embedding=audio, mask_cond_fea=static["mask_cond"],
                          full_mask=static["full"], face_mask=static["face"], lip_mask=static["lip"],
                          motion_scale=motion_scale, banks=unet._banks)
-        eng.set_schedule(timesteps.tolist(), coef_table_of(self.scheduler), guidance_scale)
+        sampler, table = sampler_table_of(self.scheduler)
+        eng.set_schedule(timesteps.tolist(), table, guidance_scale, sampler)
         frames = list(eng.shard.frames)
         eng.latents.copy_(latents[:, :, frames].float())
         if self.use_cuda_graph and callback is None and eng.graph is None:

@@ -825,6 +825,38 @@ __global__ void cfg_ddim_kernel(const T* __restrict__ model_out, long long ldm,
   }
 }
 
+// CFG combine + DPM-Solver++ (order 1 or 2, data prediction) update, one table row per step:
+//   v = v_u + s (v_c - v_u);  x0 = alpha x - sigma v;  x <- a x + b x0 + c x0_prev;  x0_prev <- x0
+// coef row = [alpha, sigma, a, b, c].  Rows with c == 0 (first-order steps, among them step 0 of every window) never
+// read x0_hist: it is uninitialised there, and 0 * NaN would be NaN.  Same layouts and grid as cfg_ddim_kernel.
+template <typename T>
+__global__ void cfg_multistep_kernel(const T* __restrict__ model_out, long long ldm,
+                                     float* __restrict__ lat, float* __restrict__ x0_hist,
+                                     const float* __restrict__ coef, const int* __restrict__ step, float guidance,
+                                     int Cl, int F, int HW) {
+  pdl_wait();
+  pdl_launch();
+  const long long total = (long long)F * HW;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const float* cf = coef + 5 * (*step);
+  const float sa = cf[0], sb = cf[1], ca = cf[2], cb = cf[3], cc = cf[4];
+  const int f = (int)(i / HW);
+  const int p = (int)(i - (long long)f * HW);
+  for (int c = 0; c < Cl; ++c) {
+    const float vu = Cvt<T>::to_f(model_out[i * ldm + c]);
+    const float vc = Cvt<T>::to_f(model_out[(total + i) * ldm + c]);
+    const float v = vu + guidance * (vc - vu);
+    const long long o = ((long long)c * F + f) * HW + p;
+    const float x = lat[o];
+    const float x0 = sa * x - sb * v;
+    float xn = ca * x + cb * x0;
+    if (cc != 0.f) xn += cc * x0_hist[o];
+    lat[o] = xn;
+    x0_hist[o] = x0;
+  }
+}
+
 __global__ void advance_step_kernel(int* step, int n_steps) {
   pdl_wait();
   pdl_launch();
@@ -1164,6 +1196,21 @@ extern "C" int hallo_b200_cfg_ddim_step(int dtype, const void* model_out, int64_
   HB_DISPATCH_T(dtype, {
     launch_kernel(cfg_ddim_kernel<T>, (int)((total + 127) / 128), 128, 0, s, (const T*)model_out, ldm, latents, coef,
                                                                   step, guidance, Cl, F, HW, v_out);
+  })
+  HB_LAUNCH_CHECK();
+  return HB_OK;
+}
+
+extern "C" int hallo_b200_cfg_multistep_step(int dtype, const void* model_out, int64_t ldm, float* latents,
+                                             float* x0_hist, const float* coef, const int32_t* step, float guidance,
+                                             int Cl, int F, int HW, hb_stream_t stream) {
+  if (!model_out || !latents || !x0_hist || !coef || !step)
+    return fail(HB_ERR_NULL, "cfg_multistep_step: null pointer");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const long long total = (long long)F * HW;
+  HB_DISPATCH_T(dtype, {
+    launch_kernel(cfg_multistep_kernel<T>, (int)((total + 127) / 128), 128, 0, s, (const T*)model_out, ldm, latents,
+                  x0_hist, coef, step, guidance, Cl, F, HW);
   })
   HB_LAUNCH_CHECK();
   return HB_OK;

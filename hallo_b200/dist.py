@@ -118,9 +118,10 @@ def sharded_vs_unsharded(eng, inp: dict, steps: int = 2, use_graph: bool = False
     full = torch.cat(parts, dim=2)                                        # frame groups in rank order
     ref = DenoiseEngine(eng.W, eng.h, eng.w, eng.f, Shard(frames=tuple(range(eng.f))))
     ref.begin_window(**window_inputs_to_device(inp, eng.dev, eng.dtype))
-    ref.n_steps, ref.guidance = eng.n_steps, eng.guidance
+    ref.n_steps, ref.guidance, ref.sampler = eng.n_steps, eng.guidance, eng.sampler
     ref.t_table.copy_(eng.t_table)
     ref.coef.copy_(eng.coef)
+    ref.coef_ms.copy_(eng.coef_ms)
     ref.latents.copy_(lat0.to(eng.dev))
     for _ in range(steps):
         ref.step()

@@ -213,11 +213,15 @@ class DenoiseEngine:
         self.MAX_STEPS = 1024
         self.t_table = torch.zeros(self.MAX_STEPS, dtype=torch.float32, device=self.dev)
         self.coef = torch.zeros(self.MAX_STEPS, 4, dtype=torch.float32, device=self.dev)
+        # DPM-Solver++ rows [alpha, sigma, a, b, c] and the previous step's data estimate (x0_hist, set up below)
+        self.coef_ms = torch.zeros(self.MAX_STEPS, 5, dtype=torch.float32, device=self.dev)
+        self.sampler = "ddim"                            # "ddim" (coef) or "multistep" (coef_ms + x0_hist)
         self.n_steps = 1
         self.guidance = 1.0
-        self._captured_with = None                       # (n_steps, guidance) baked into the graph as kernel arguments
+        self._captured_with = None           # (n_steps, guidance, sampler) baked into the graph: kernel arguments / choice
         assert self.nm + n_frames <= self.cfg.pe_max_len, "temporal length exceeds the positional-encoding table"
         self.latents = torch.zeros(1, self.cfg.in_channels, self.fl, h, w, dtype=torch.float32, device=self.dev)
+        self.x0_hist = torch.zeros_like(self.latents)
         self.model_out: Optional[torch.Tensor] = None
         self.sample: Optional[torch.Tensor] = None      # per-half fp32 sample for the plain forward() API path
         # frame-sharded window: R ranks (or an emulated R on one GPU) swap frame <-> pixel ownership around motion modules
@@ -418,17 +422,26 @@ class DenoiseEngine:
             self.arena.barrier()
         torch.cuda.current_stream().synchronize()
 
-    def set_schedule(self, timesteps: Sequence[int], coef: torch.Tensor, guidance: float):
+    def set_schedule(self, timesteps: Sequence[int], coef: torch.Tensor, guidance: float, sampler: str = "ddim"):
         """Per-window schedule.  The tables keep their device addresses (a captured graph reads them); the step count
-        and the guidance scale are kernel ARGUMENTS of the captured launches, so changing them drops the graph."""
+        and the guidance scale are kernel ARGUMENTS of the captured launches and the sampler chooses the step kernel,
+        so changing any of them drops the graph.  sampler "ddim": coef is the [n, 4] DDIM table
+        (scheduler.coef_table_of); "multistep": the [n, 5] DPM-Solver++ table (scheduler.sampler_table_of).  Row 0 of
+        a multistep table is first order, so a new window needs no reset of the x0 history."""
         n = len(timesteps)
         if n > self.MAX_STEPS:
             raise ValueError(f"{n} inference steps exceed the engine's schedule capacity ({self.MAX_STEPS})")
+        width = {"ddim": 4, "multistep": 5}.get(sampler)
+        if width is None:
+            raise ValueError(f"unknown sampler {sampler!r} (ddim, multistep)")
+        if coef.numel() != n * width:
+            raise ValueError(f"a {n}-step {sampler} schedule needs a [{n}, {width}] table, got {tuple(coef.shape)}")
         self.n_steps = n
         self.t_table[:n].copy_(torch.tensor([float(t) for t in timesteps], dtype=torch.float32))
-        self.coef[:n].copy_(coef.to(torch.float32).reshape(n, 4))
+        (self.coef if sampler == "ddim" else self.coef_ms)[:n].copy_(coef.to(torch.float32).reshape(n, width))
+        self.sampler = sampler
         self.guidance = float(guidance)
-        if self.graph is not None and self._captured_with != (self.n_steps, self.guidance):
+        if self.graph is not None and self._captured_with != (self.n_steps, self.guidance, self.sampler):
             self.graph = None
         self.step_idx.zero_()
 
@@ -754,9 +767,12 @@ class DenoiseEngine:
 
     @torch.no_grad()
     def _step_tail(self):
-        """CFG combine + DDIM update + step counter (face_animate.py:415-420)."""
+        """CFG combine + scheduler update (DDIM or DPM-Solver++) + step counter (face_animate.py:415-420)."""
         mo = self.model_out                    # both CFG halves of the local frames: the combine is rank-local
-        ops.cfg_ddim_step(mo, self.latents, self.coef, self.step_idx, guidance=self.guidance)
+        if self.sampler == "multistep":
+            ops.cfg_multistep_step(mo, self.latents, self.x0_hist, self.coef_ms, self.step_idx, guidance=self.guidance)
+        else:
+            ops.cfg_ddim_step(mo, self.latents, self.coef, self.step_idx, guidance=self.guidance)
         ops.advance_step(self.step_idx, self.n_steps)
 
     # ------------------------------------------------------------------ public
@@ -780,9 +796,10 @@ class DenoiseEngine:
 
     @torch.no_grad()
     def capture(self):
-        """Warm up (allocates every buffer) and capture forward + CFG/DDIM step into one CUDA graph."""
+        """Warm up (allocates every buffer) and capture forward + CFG/scheduler step into one CUDA graph."""
         lat0 = self.latents.clone()
         st0 = self.step_idx.clone()
+        hist0 = self.x0_hist.clone()                     # a capture between steps of a multistep schedule keeps its history
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
@@ -792,13 +809,14 @@ class DenoiseEngine:
         torch.cuda.synchronize()
         self.latents.copy_(lat0)
         self.step_idx.copy_(st0)
+        self.x0_hist.copy_(hist0)
         g = torch.cuda.CUDAGraph()
         # thread_local: the NCCL watchdog thread may touch CUDA while this thread captures (multi-GPU shards)
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
             self._forward()
             self._step_tail()
         self.graph = g
-        self._captured_with = (self.n_steps, self.guidance)
+        self._captured_with = (self.n_steps, self.guidance, self.sampler)
         self.latents.copy_(lat0)
         self.step_idx.copy_(st0)
 

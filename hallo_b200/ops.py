@@ -423,6 +423,23 @@ def cfg_ddim_step(model_out: torch.Tensor, latents: torch.Tensor, coef: torch.Te
     return latents
 
 
+@_timed(lambda *a, **kw: "cfg_multistep_step")
+def cfg_multistep_step(model_out: torch.Tensor, latents: torch.Tensor, x0_hist: torch.Tensor, coef: torch.Tensor,
+                       step: torch.Tensor, *, guidance: float) -> torch.Tensor:
+    """DPM-Solver++ step.  model_out: [2*F*HW, ld] tokens (uncond rows then cond rows); latents: fp32 [1, Cl, F, H, W]
+    updated in place; x0_hist: fp32 like latents, the previous step's data estimate, overwritten with this step's;
+    coef: fp32 [n_steps, 5] rows [alpha, sigma, a, b, c] (hallo_b200.scheduler.DPMSolverMultistepScheduler)."""
+    _, cl, f, h, w = latents.shape
+    assert latents.dtype == torch.float32 and latents.is_contiguous()
+    assert x0_hist.dtype == torch.float32 and x0_hist.is_contiguous() and x0_hist.shape == latents.shape
+    assert coef.dtype == torch.float32 and coef.is_contiguous() and coef.shape[-1] == 5
+    lib.check(lib.load().hallo_b200_cfg_multistep_step(
+        _i(lib.dtype_code(model_out.dtype)), C.c_void_p(lib.ptr(model_out)), C.c_int64(_rowmajor_ld(model_out)),
+        C.c_void_p(lib.ptr(latents)), C.c_void_p(lib.ptr(x0_hist)), C.c_void_p(lib.ptr(coef)), C.c_void_p(lib.ptr(step)),
+        C.c_float(guidance), _i(cl), _i(f), _i(h * w), lib.current_stream()), "cfg_multistep_step")
+    return latents
+
+
 def advance_step(step: torch.Tensor, n_steps: int) -> None:
     lib.check(lib.load().hallo_b200_advance_step(C.c_void_p(lib.ptr(step)), _i(n_steps), lib.current_stream()),
               "advance_step")

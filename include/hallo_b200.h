@@ -276,6 +276,13 @@ int hallo_b200_timestep_embed(int dtype, const float* t_table, const int32_t* st
 int hallo_b200_cfg_ddim_step(int dtype, const void* model_out, int64_t ldm, float* latents, const float* coef,
                              const int32_t* step, float guidance, int Cl, int F, int HW, float* v_out,
                              hb_stream_t stream);
+/* CFG combine + DPM-Solver++ (order 1 or 2, data prediction) v-prediction update on fp32 latents [1, Cl, F, HW].
+ * coef: fp32 [n_steps, 5] = alpha, sigma, a, b, c; with v = v_u + guidance (v_c - v_u) and x0 = alpha x - sigma v,
+ * x <- a x + b x0 + c x0_hist, then x0_hist <- x0.  x0_hist: fp32, shaped like latents; it is not read on rows with
+ * c == 0, so step 0 of a schedule needs no initialised history. */
+int hallo_b200_cfg_multistep_step(int dtype, const void* model_out, int64_t ldm, float* latents, float* x0_hist,
+                                  const float* coef, const int32_t* step, float guidance, int Cl, int F, int HW,
+                                  hb_stream_t stream);
 int hallo_b200_advance_step(int32_t* step, int n_steps, hb_stream_t stream);
 /* channels-last [B*F*HW, ld] (first C columns) -> fp32 [B, C, F, HW] (the reference's output layout). */
 int hallo_b200_tokens_to_bcfhw(int dtype, const void* x, int64_t ld, float* out, int B, int C, int F, int HW,
