@@ -887,6 +887,50 @@ __global__ void cfg_ancestral_kernel(const T* __restrict__ model_out, long long 
   }
 }
 
+// CFG combine + UniPC (bh1 / bh2, order 1 or 2, data prediction) update, one table row per step:
+//   v = v_u + s (v_c - v_u);  m = alpha x - sigma v             (data estimate at the sample the UNet saw)
+//   c = kx x + kL L + k0 m + k1 m1 + k2 m2                      (UniC corrector; kx = 1 and the rest 0 on rows without it)
+//   x <- pc c + p0 m + p1 m1;  L <- c;  m2 <- m1;  m1 <- m      (UniP predictor, then the history moves one step)
+// coef row = [alpha, sigma, kx, kL, k0, k1, k2, pc, p0, p1].  A term with a zero coefficient never reads its buffer:
+// L, m1 and m2 are uninitialised on the first rows of a window, and 0 * NaN would be NaN.  m1 is always read, since it
+// moves into m2, but only enters the arithmetic when k1 or p1 is nonzero.  Same layouts and grid as cfg_ddim_kernel.
+template <typename T>
+__global__ void cfg_unipc_kernel(const T* __restrict__ model_out, long long ldm, float* __restrict__ lat,
+                                 float* __restrict__ last, float* __restrict__ m1_hist, float* __restrict__ m2_hist,
+                                 const float* __restrict__ coef, const int* __restrict__ step, float guidance,
+                                 int Cl, int F, int HW) {
+  pdl_wait();
+  pdl_launch();
+  const long long total = (long long)F * HW;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const float* cf = coef + 10 * (*step);
+  const float sa = cf[0], sb = cf[1], kx = cf[2], kl = cf[3], k0 = cf[4], k1 = cf[5], k2 = cf[6];
+  const float pc = cf[7], p0 = cf[8], p1 = cf[9];
+  const int f = (int)(i / HW);
+  const int p = (int)(i - (long long)f * HW);
+  for (int c = 0; c < Cl; ++c) {
+    const float vu = Cvt<T>::to_f(model_out[i * ldm + c]);
+    const float vc = Cvt<T>::to_f(model_out[(total + i) * ldm + c]);
+    const float v = vu + guidance * (vc - vu);
+    const long long o = ((long long)c * F + f) * HW + p;
+    const float x = lat[o];
+    const float m = sa * x - sb * v;
+    const float m1 = m1_hist[o];
+    float cr = k0 * m;
+    if (kx != 0.f) cr += kx * x;
+    if (kl != 0.f) cr += kl * last[o];
+    if (k1 != 0.f) cr += k1 * m1;
+    if (k2 != 0.f) cr += k2 * m2_hist[o];
+    float xn = pc * cr + p0 * m;
+    if (p1 != 0.f) xn += p1 * m1;
+    lat[o] = xn;
+    last[o] = cr;
+    m2_hist[o] = m1;
+    m1_hist[o] = m;
+  }
+}
+
 __global__ void advance_step_kernel(int* step, int n_steps) {
   pdl_wait();
   pdl_launch();
@@ -1256,6 +1300,22 @@ extern "C" int hallo_b200_cfg_ancestral_step(int dtype, const void* model_out, i
   HB_DISPATCH_T(dtype, {
     launch_kernel(cfg_ancestral_kernel<T>, (int)((total + 127) / 128), 128, 0, s, (const T*)model_out, ldm, latents,
                   (const T*)noise, coef, step, guidance, Cl, F, HW);
+  })
+  HB_LAUNCH_CHECK();
+  return HB_OK;
+}
+
+extern "C" int hallo_b200_cfg_unipc_step(int dtype, const void* model_out, int64_t ldm, float* latents,
+                                         float* last_sample, float* x0_hist, float* x0_hist2, const float* coef,
+                                         const int32_t* step, float guidance, int Cl, int F, int HW,
+                                         hb_stream_t stream) {
+  if (!model_out || !latents || !last_sample || !x0_hist || !x0_hist2 || !coef || !step)
+    return fail(HB_ERR_NULL, "cfg_unipc_step: null pointer");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const long long total = (long long)F * HW;
+  HB_DISPATCH_T(dtype, {
+    launch_kernel(cfg_unipc_kernel<T>, (int)((total + 127) / 128), 128, 0, s, (const T*)model_out, ldm, latents,
+                  last_sample, x0_hist, x0_hist2, coef, step, guidance, Cl, F, HW);
   })
   HB_LAUNCH_CHECK();
   return HB_OK;

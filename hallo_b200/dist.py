@@ -127,6 +127,7 @@ def sharded_vs_unsharded(eng, inp: dict, steps: int = 2, use_graph: bool = False
     ref.t_table.copy_(eng.t_table)
     ref.coef.copy_(eng.coef)
     ref.coef_ms.copy_(eng.coef_ms)
+    ref.coef_uni.copy_(eng.coef_uni)
     if noise is not None:
         ref.set_noise(noise)
     ref.latents.copy_(lat0.to(eng.dev))

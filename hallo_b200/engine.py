@@ -215,7 +215,10 @@ class DenoiseEngine:
         self.coef = torch.zeros(self.MAX_STEPS, 4, dtype=torch.float32, device=self.dev)
         # DPM-Solver++ rows [alpha, sigma, a, b, c] and the previous step's data estimate (x0_hist, set up below)
         self.coef_ms = torch.zeros(self.MAX_STEPS, 5, dtype=torch.float32, device=self.dev)
-        # "ddim" (coef), "multistep" (coef_ms + x0_hist) or "ancestral" (coef_ms rows [alpha, sigma, a, b, d] + noise)
+        # UniPC rows [alpha, sigma, kx, kL, k0, k1, k2, pc, p0, p1] (scheduler.unipc_table)
+        self.coef_uni = torch.zeros(self.MAX_STEPS, 10, dtype=torch.float32, device=self.dev)
+        # "ddim" (coef), "multistep" (coef_ms + x0_hist), "ancestral" (coef_ms rows [alpha, sigma, a, b, d] + noise) or
+        # "unipc" (coef_uni + last_sample, x0_hist, x0_hist2)
         self.sampler = "ddim"
         self.noise: Optional[torch.Tensor] = None        # ancestral: [n_steps, Cl, fl, h, w] model-dtype draws, this rank's frames
         self.n_steps = 1
@@ -224,6 +227,8 @@ class DenoiseEngine:
         assert self.nm + n_frames <= self.cfg.pe_max_len, "temporal length exceeds the positional-encoding table"
         self.latents = torch.zeros(1, self.cfg.in_channels, self.fl, h, w, dtype=torch.float32, device=self.dev)
         self.x0_hist = torch.zeros_like(self.latents)
+        self.last_sample = torch.zeros_like(self.latents)      # UniPC: the previous step's corrected sample
+        self.x0_hist2 = torch.zeros_like(self.latents)         # UniPC: the data estimate of two steps back
         self.model_out: Optional[torch.Tensor] = None
         self.sample: Optional[torch.Tensor] = None      # per-half fp32 sample for the plain forward() API path
         # frame-sharded window: R ranks (or an emulated R on one GPU) swap frame <-> pixel ownership around motion modules
@@ -432,20 +437,22 @@ class DenoiseEngine:
         (scheduler.coef_table_of); "multistep": the [n, 5] DPM-Solver++ or Euler table (scheduler.sampler_table_of).
         Row 0 of a multistep table is first order, so a new window needs no reset of the x0 history.  "ancestral": the
         [n, 5] Euler-a table, and noise, this window's [n, Cl, fl, h, w] draws (see set_noise); noise may also be
-        given later through set_noise, before the first step."""
+        given later through set_noise, before the first step.  "unipc": the [n, 10] UniPC table; its row 0 has no
+        corrector and is first order, so a new window needs no reset of last_sample or the history either."""
         n = len(timesteps)
         if n > self.MAX_STEPS:
             raise ValueError(f"{n} inference steps exceed the engine's schedule capacity ({self.MAX_STEPS})")
-        width = {"ddim": 4, "multistep": 5, "ancestral": 5}.get(sampler)
+        width = {"ddim": 4, "multistep": 5, "ancestral": 5, "unipc": 10}.get(sampler)
         if width is None:
-            raise ValueError(f"unknown sampler {sampler!r} (ddim, multistep, ancestral)")
+            raise ValueError(f"unknown sampler {sampler!r} (ddim, multistep, ancestral, unipc)")
         if coef.numel() != n * width:
             raise ValueError(f"a {n}-step {sampler} schedule needs a [{n}, {width}] table, got {tuple(coef.shape)}")
         if noise is not None and sampler != "ancestral":
             raise ValueError(f"the {sampler} sampler takes no noise")
         self.n_steps = n
         self.t_table[:n].copy_(torch.tensor([float(t) for t in timesteps], dtype=torch.float32))
-        (self.coef if sampler == "ddim" else self.coef_ms)[:n].copy_(coef.to(torch.float32).reshape(n, width))
+        table = {"ddim": self.coef, "unipc": self.coef_uni}.get(sampler, self.coef_ms)
+        table[:n].copy_(coef.to(torch.float32).reshape(n, width))
         self.sampler = sampler
         self.guidance = float(guidance)
         if self.graph is not None and self._captured_with != (self.n_steps, self.guidance, self.sampler):
@@ -794,7 +801,7 @@ class DenoiseEngine:
 
     @torch.no_grad()
     def _step_tail(self):
-        """CFG combine + scheduler update (DDIM, DPM-Solver++ / Euler or Euler-a) + step counter
+        """CFG combine + scheduler update (DDIM, DPM-Solver++ / Euler, Euler-a or UniPC) + step counter
         (face_animate.py:415-420)."""
         mo = self.model_out                    # both CFG halves of the local frames: the combine is rank-local
         if self.sampler == "multistep":
@@ -803,6 +810,9 @@ class DenoiseEngine:
             if self.noise is None or self.noise.shape[0] != self.n_steps:
                 raise RuntimeError("the ancestral sampler needs this window's noise (set_noise) before it steps")
             ops.cfg_ancestral_step(mo, self.latents, self.noise, self.coef_ms, self.step_idx, guidance=self.guidance)
+        elif self.sampler == "unipc":
+            ops.cfg_unipc_step(mo, self.latents, self.last_sample, self.x0_hist, self.x0_hist2, self.coef_uni,
+                               self.step_idx, guidance=self.guidance)
         else:
             ops.cfg_ddim_step(mo, self.latents, self.coef, self.step_idx, guidance=self.guidance)
         ops.advance_step(self.step_idx, self.n_steps)
@@ -829,9 +839,9 @@ class DenoiseEngine:
     @torch.no_grad()
     def capture(self):
         """Warm up (allocates every buffer) and capture forward + CFG/scheduler step into one CUDA graph."""
-        lat0 = self.latents.clone()
-        st0 = self.step_idx.clone()
-        hist0 = self.x0_hist.clone()                     # a capture between steps of a multistep schedule keeps its history
+        # the warm-up runs one real step: a capture between steps of a multistep schedule keeps every piece of state
+        state = (self.latents, self.step_idx, self.x0_hist, self.last_sample, self.x0_hist2)
+        saved = [t.clone() for t in state]
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
@@ -839,9 +849,8 @@ class DenoiseEngine:
             self._step_tail()
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
-        self.latents.copy_(lat0)
-        self.step_idx.copy_(st0)
-        self.x0_hist.copy_(hist0)
+        for t, t0 in zip(state, saved):
+            t.copy_(t0)
         g = torch.cuda.CUDAGraph()
         # thread_local: the NCCL watchdog thread may touch CUDA while this thread captures (multi-GPU shards)
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
@@ -849,8 +858,8 @@ class DenoiseEngine:
             self._step_tail()
         self.graph = g
         self._captured_with = (self.n_steps, self.guidance, self.sampler)
-        self.latents.copy_(lat0)
-        self.step_idx.copy_(st0)
+        for t, t0 in zip(state, saved):
+            t.copy_(t0)
 
     @torch.no_grad()
     def step(self):

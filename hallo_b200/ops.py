@@ -457,6 +457,26 @@ def cfg_ancestral_step(model_out: torch.Tensor, latents: torch.Tensor, noise: to
     return latents
 
 
+@_timed(lambda *a, **kw: "cfg_unipc_step")
+def cfg_unipc_step(model_out: torch.Tensor, latents: torch.Tensor, last_sample: torch.Tensor, x0_hist: torch.Tensor,
+                   x0_hist2: torch.Tensor, coef: torch.Tensor, step: torch.Tensor, *, guidance: float) -> torch.Tensor:
+    """UniPC step (corrector, then predictor).  model_out: [2*F*HW, ld] tokens (uncond rows then cond rows); latents:
+    fp32 [1, Cl, F, H, W] updated in place; last_sample, x0_hist, x0_hist2: fp32 like latents, the previous corrected
+    sample and the two previous data estimates, moved on by one step; coef: fp32 [n_steps, 10] rows
+    [alpha, sigma, kx, kL, k0, k1, k2, pc, p0, p1] (hallo_b200.scheduler.unipc_table)."""
+    _, cl, f, h, w = latents.shape
+    assert latents.dtype == torch.float32 and latents.is_contiguous()
+    for t in (last_sample, x0_hist, x0_hist2):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.shape == latents.shape
+    assert coef.dtype == torch.float32 and coef.is_contiguous() and coef.shape[-1] == 10
+    lib.check(lib.load().hallo_b200_cfg_unipc_step(
+        _i(lib.dtype_code(model_out.dtype)), C.c_void_p(lib.ptr(model_out)), C.c_int64(_rowmajor_ld(model_out)),
+        C.c_void_p(lib.ptr(latents)), C.c_void_p(lib.ptr(last_sample)), C.c_void_p(lib.ptr(x0_hist)),
+        C.c_void_p(lib.ptr(x0_hist2)), C.c_void_p(lib.ptr(coef)), C.c_void_p(lib.ptr(step)), C.c_float(guidance),
+        _i(cl), _i(f), _i(h * w), lib.current_stream()), "cfg_unipc_step")
+    return latents
+
+
 def advance_step(step: torch.Tensor, n_steps: int) -> None:
     lib.check(lib.load().hallo_b200_advance_step(C.c_void_p(lib.ptr(step)), _i(n_steps), lib.current_stream()),
               "advance_step")

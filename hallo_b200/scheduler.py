@@ -15,6 +15,10 @@ EulerDiscreteScheduler and EulerAncestralDiscreteScheduler ("Euler", "Euler a") 
 names (release 0.27.2).  They work on x = y / alpha; the engine keeps y, so their tables are in the VP form (see
 euler_table) and `latent_scales_of` converts between the two.  Euler runs on the multistep kernel; Euler-a on
 `hallo_b200_cfg_ancestral_step`, with its per-step noise drawn on the host from the caller's generator.
+
+UniPCMultistepScheduler is UniPC (bh1 / bh2, order 1 or 2, data prediction), diffusers' usual few-step sampler for
+SD-family models.  Its corrector reuses the UNet evaluation the next step needs, so a step is still one forward; the
+corrector and predictor together are one [n, 10] table row (unipc_table) for `hallo_b200_cfg_unipc_step`.
 """
 from __future__ import annotations
 
@@ -172,6 +176,49 @@ def dpm_solver_table(alpha: Sequence[float], sigma: Sequence[float], second_orde
     return torch.from_numpy(rows).to(torch.float32)
 
 
+def _solver_alphas_cumprod(num_train_timesteps: int, beta_start: float, beta_end: float, beta_schedule: str,
+                           rescale_betas_zero_snr: bool) -> torch.Tensor:
+    """alpha_cumprod of the training schedule for the multistep solvers (DPM-Solver++, UniPC): DDIM's, with the
+    zero-terminal-SNR value alpha_cumprod[-1] = 0 replaced by 2^-24, as diffusers does, so lambda stays finite."""
+    ac = DDIMScheduler(num_train_timesteps, beta_start, beta_end, beta_schedule,
+                       rescale_betas_zero_snr=rescale_betas_zero_snr).alphas_cumprod.clone()
+    if rescale_betas_zero_snr:
+        ac[-1] = 2.0 ** -24
+    return ac
+
+
+def _solver_timesteps(n: int, T: int, spacing: str, steps_offset: int) -> np.ndarray:
+    """int64 [n] timesteps of the multistep solvers for "trailing", "leading" or "linspace" spacing (diffusers'
+    DPMSolverMultistepScheduler / UniPCMultistepScheduler rule, which differs from DDIM's for "leading")."""
+    if spacing == "trailing":
+        ts = np.round(np.arange(T, 0, -T / n)) - 1
+    elif spacing == "leading":
+        ts = (np.arange(0, n + 1) * (T // (n + 1))).round()[::-1][:-1] + steps_offset
+    else:
+        ts = np.linspace(0, T - 1, n + 1).round()[::-1][:-1]
+    return ts.astype(np.int64).copy()
+
+
+def _solver_points(alphas_cumprod: torch.Tensor, ts: np.ndarray, final_sigmas_type: str):
+    """float64 alpha, sigma at the n step points, then the final point: abar = 1 ("zero") or alpha_cumprod[0]
+    ("sigma_min")."""
+    ac = alphas_cumprod.double().numpy()
+    abar = np.append(ac[ts], 1.0 if final_sigmas_type == "zero" else ac[0])
+    return np.sqrt(abar), np.sqrt(1.0 - abar)
+
+
+def _points_from_sigmas(sched, what: str):
+    """float64 alpha, sigma of a diffusers-style solver object from its own n + 1 sigmas = sigma / alpha."""
+    n = len(sched.timesteps)
+    s = torch.as_tensor(sched.sigmas).detach().cpu().double().numpy()
+    if len(s) != n + 1:
+        raise ValueError(f"a {n}-step {what} schedule needs {n + 1} sigmas, got {len(s)}")
+    al = 1.0 / np.sqrt(1.0 + s * s)
+    with np.errstate(invalid="ignore"):
+        sg = np.where(np.isinf(s), 1.0, s * al)                   # sigma / alpha = inf: alpha = 0, sigma = 1
+    return al, sg
+
+
 def _check_dpm_config(get) -> None:
     """NotImplementedError, naming the setting, for DPMSolverMultistepScheduler settings the engine does not run."""
     order = int(get("solver_order", 2))
@@ -215,11 +262,8 @@ class DPMSolverMultistepScheduler:
             raise NotImplementedError(f"final_sigmas_type {final_sigmas_type!r}")
         if timestep_spacing not in ("trailing", "leading", "linspace"):
             raise NotImplementedError(timestep_spacing)
-        ac = DDIMScheduler(num_train_timesteps, beta_start, beta_end, beta_schedule,
-                           rescale_betas_zero_snr=rescale_betas_zero_snr).alphas_cumprod.clone()
-        if rescale_betas_zero_snr:
-            ac[-1] = 2.0 ** -24
-        self.alphas_cumprod = ac
+        self.alphas_cumprod = _solver_alphas_cumprod(num_train_timesteps, beta_start, beta_end, beta_schedule,
+                                                     rescale_betas_zero_snr)
         self.num_train_timesteps = num_train_timesteps
         self.solver_order, self.solver_type = int(solver_order), solver_type
         self.lower_order_final, self.euler_at_final = lower_order_final, euler_at_final
@@ -232,19 +276,11 @@ class DPMSolverMultistepScheduler:
         self._x0_prev: Optional[torch.Tensor] = None
 
     def set_timesteps(self, num_inference_steps: int, device=None):
-        n, T = num_inference_steps, self.num_train_timesteps
-        if self.timestep_spacing == "trailing":
-            ts = np.round(np.arange(T, 0, -T / n)) - 1
-        elif self.timestep_spacing == "leading":
-            ts = (np.arange(0, n + 1) * (T // (n + 1))).round()[::-1][:-1] + self.steps_offset
-        else:
-            ts = np.linspace(0, T - 1, n + 1).round()[::-1][:-1]
-        ts = ts.astype(np.int64)
+        n = num_inference_steps
+        ts = _solver_timesteps(n, self.num_train_timesteps, self.timestep_spacing, self.steps_offset)
         self.num_inference_steps = n
-        self.timesteps = torch.from_numpy(ts.copy()).to(device)
-        ac = self.alphas_cumprod.double().numpy()
-        abar = np.append(ac[ts], 1.0 if self.final_sigmas_type == "zero" else ac[0])
-        self._alpha, self._sigma = np.sqrt(abar), np.sqrt(1.0 - abar)       # step points, then the final point
+        self.timesteps = torch.from_numpy(ts).to(device)
+        self._alpha, self._sigma = _solver_points(self.alphas_cumprod, ts, self.final_sigmas_type)
         self.sigmas = torch.from_numpy(self._sigma / self._alpha).to(torch.float32)
         self._second = dpm_second_order_steps(n, self.solver_order, self.lower_order_final, self.euler_at_final,
                                               self.final_sigmas_type)
@@ -479,10 +515,272 @@ class EulerAncestralDiscreteScheduler(EulerDiscreteScheduler):
     _ancestral = True
 
 
+# ----------------------------------------------------------------------------------------------------------- UniPC
+# UniPC (Zhao et al. 2023, arXiv:2302.04867) in data prediction: step i sees the sample s_i the UNet ran on, forms
+# m_i = alpha_i s_i - sigma_i v_i, corrects the sample with the new m_i (UniC, reusing the evaluation the next step
+# needs anyway), then predicts s_{i+1} from the corrected sample (UniP).  Both are linear in the sample, the previous
+# corrected sample L and the data estimates m_i, m_{i-1}, m_{i-2}, so each step is one table row.
+def unipc_orders(n: int, solver_order: int, lower_order_final: bool = True) -> List[int]:
+    """The order of each of n steps by diffusers' rule: min(solver_order, i + 1), and with lower_order_final also at
+    most n - i, so the last step is first order whatever n is (unlike DPM-Solver++, which lowers it below 15 steps)."""
+    return [min(solver_order, n - i if lower_order_final else solver_order, i + 1) for i in range(n)]
+
+
+def _unipc_bh(h: float, solver_type: str) -> float:
+    """B(h) of the bh1 / bh2 variants, with hh = -h (data prediction)."""
+    return -h if solver_type == "bh1" else float(np.expm1(-h))
+
+
+def unipc_table(alpha: Sequence[float], sigma: Sequence[float], disable_corrector: Sequence[int] = (),
+                solver_order: int = 2, solver_type: str = "bh2", lower_order_final: bool = True) -> torch.Tensor:
+    """[n, 10] rows [alpha_i, sigma_i, kx, kL, k0, k1, k2, pc, p0, p1] of UniPC (data prediction, order 1 or 2, bh1
+    or bh2), for the engine's step s -> s' with m_i = alpha_i s - sigma_i v:
+      corrector  c = kx s + kL L + k0 m_i + k1 m_{i-1} + k2 m_{i-2}  (kx = 1, the rest 0 at i = 0, where i - 1 is in
+                 disable_corrector; otherwise kx = 0 and L is the previous step's corrected sample)
+      predictor  s' = pc c + p0 m_i + p1 m_{i-1}
+    alpha, sigma: the n step points, then the final point.  With lambda = log alpha - log sigma, the update from point
+    a to point b (h = lambda_b - lambda_a) is (sigma_b / sigma_a) x + E m_a - alpha_b B(h) sum rho_k D_k, where
+    E = alpha_b (1 - e^{-h}), B(h) = -h (bh1) or e^{-h} - 1 (bh2), and D_k the scaled differences of diffusers'
+    multistep_uni_p_bh_update / multistep_uni_c_bh_update.  The predictor of order 2 uses rho = 0.5, as diffusers
+    hard-codes; the corrector uses rho = 0.5 at order 1 and solves diffusers' 2 x 2 system R rho = b at order 2.  The
+    corrector at step i has the order of step i - 1's predictor.  Computed in float64 and stored as fp32.
+    The limits are taken where they are reached: alpha_0 = 0 (lambda_0 = -inf) gives E = alpha_1 and drops every
+    difference against point 0 (its r_k is infinite); sigma_n = 0 gives pc = 0 and p0 = alpha_n at first order.  A
+    second-order last step onto sigma = 0 (r_k -> 0) and bh1's corrector after alpha_0 = 0 (B = -inf) have no finite
+    limit and raise NotImplementedError."""
+    al, sg = np.asarray(alpha, np.float64), np.asarray(sigma, np.float64)
+    n = len(al) - 1
+    if len(sg) != n + 1 or n < 1:
+        raise ValueError(f"{len(al)} alphas and {len(sg)} sigmas do not describe a UniPC schedule")
+    if solver_type not in ("bh1", "bh2"):
+        raise NotImplementedError(f"solver_type {solver_type!r}: the engine runs UniPC 'bh1' and 'bh2'")
+    if solver_order not in (1, 2):
+        raise NotImplementedError(f"solver_order {solver_order}: the engine runs UniPC of order 1 or 2")
+    orders = unipc_orders(n, solver_order, lower_order_final)
+    if orders[-1] == 2 and sg[n] == 0.0:
+        raise NotImplementedError("lower_order_final=False with a final sigma of 0 (final_sigmas_type='zero'): a "
+                                  "second-order UniPC step onto sigma = 0 diverges; keep lower_order_final=True")
+    with np.errstate(divide="ignore"):
+        lam = np.log(al) - np.log(sg)
+    skip = {int(k) for k in disable_corrector}
+
+    def base(a, b):
+        """sigma_b / sigma_a and E = alpha_b (1 - e^{-h}) = alpha_b - (sigma_b / sigma_a) alpha_a (finite at both ends)."""
+        r = sg[b] / sg[a]
+        return r, al[b] - r * al[a]
+
+    def inv_rk(prev, a, h):
+        """1 / r_k, r_k = (lambda_prev - lambda_a) / h; 0 where lambda_prev = -inf."""
+        return 0.0 if np.isinf(lam[prev]) else h / (lam[prev] - lam[a])
+
+    rows = np.zeros((n, 10), np.float64)
+    for i in range(n):
+        kx, kl, k0, k1, k2 = 1.0, 0.0, 0.0, 0.0, 0.0
+        if i > 0 and (i - 1) not in skip:                          # UniC: from point i - 1 to i, with m_i
+            kx = 0.0
+            kl, e = base(i - 1, i)
+            h = lam[i] - lam[i - 1]
+            bh = _unipc_bh(h, solver_type)
+            if not np.isfinite(bh):
+                raise NotImplementedError(f"solver_type {solver_type!r} with alpha = 0 at step point {i - 1}: the "
+                                          "corrector's B(h) is infinite; use 'bh2' or an alpha_cumprod above 0")
+            if orders[i - 1] == 1:
+                rho_t, rho_p_rk = 0.5, 0.0
+            else:
+                hh = -h
+                phi = np.expm1(hh) / hh - 1.0                      # h_phi_k at k = 1, then k = 2
+                b1 = phi / bh
+                b2 = (phi / hh - 0.5) * 2.0 / bh
+                q = inv_rk(i - 2, i - 1, h)
+                if q == 0.0:                                       # r_k = -inf: rho_0 -> 0, rho_t -> b1
+                    rho_t, rho_p_rk = b1, 0.0
+                else:                                              # solve [[1, 1], [r_k, 1]] rho = [b1, b2]
+                    rk = 1.0 / q
+                    rho0 = (b2 - b1) / (rk - 1.0)
+                    rho_t, rho_p_rk = b1 - rho0, rho0 * q
+            k0 = -al[i] * bh * rho_t
+            k2 = -al[i] * bh * rho_p_rk
+            k1 = e - k0 - k2
+        pc, e = base(i, i + 1)                                     # UniP: from point i to i + 1, with the corrected c
+        p0, p1 = e, 0.0
+        if orders[i] == 2:
+            h = lam[i + 1] - lam[i]
+            p1 = -al[i + 1] * _unipc_bh(h, solver_type) * 0.5 * inv_rk(i - 1, i, h)
+            p0 = e - p1
+        rows[i] = (al[i], sg[i], kx, kl, k0, k1, k2, pc, p0, p1)
+    if not np.isfinite(rows).all():
+        raise ValueError(f"UniPC rows {sorted(set(np.nonzero(~np.isfinite(rows))[0].tolist()))} are not finite: "
+                         "the schedule repeats a point or ends above its start")
+    return torch.from_numpy(rows).to(torch.float32)
+
+
+def _check_unipc_config(get) -> None:
+    """NotImplementedError, naming the setting, for UniPCMultistepScheduler settings the engine does not run."""
+    if not get("predict_x0", True):
+        raise NotImplementedError("predict_x0=False: the engine runs UniPC in data prediction (predict_x0=True)")
+    order = int(get("solver_order", 2))
+    if order not in (1, 2):
+        raise NotImplementedError(f"solver_order {order}: the engine runs UniPC of order 1 or 2")
+    st = get("solver_type", "bh2")
+    if st not in ("bh1", "bh2"):
+        raise NotImplementedError(f"solver_type {st!r}: the engine runs UniPC 'bh1' and 'bh2'")
+    if get("thresholding", False):
+        raise NotImplementedError("thresholding: dynamic thresholding of x0 is not implemented")
+    pred = get("prediction_type", None)
+    if pred not in (None, "v_prediction"):
+        raise NotImplementedError(f"prediction_type {pred!r}: the engine's update is the v-prediction form")
+    for k in ("use_karras_sigmas", "use_exponential_sigmas", "use_beta_sigmas", "use_flow_sigmas"):
+        if get(k, False):
+            raise NotImplementedError(f"{k}: only the training sigmas at the chosen timesteps are implemented")
+    if get("solver_p", None) is not None:
+        raise NotImplementedError("solver_p: an external predictor scheduler is not implemented")
+
+
+class UniPCMultistepScheduler:
+    """UniPC (bh1 / bh2, order 1 or 2, data prediction, v-prediction model) with the constructor keywords of
+    diffusers.UniPCMultistepScheduler and the DDIM keywords the reference passes.  step() restates the update of
+    diffusers 0.27.2, the release the reference pins (step / multistep_uni_c_bh_update / multistep_uni_p_bh_update,
+    order-2 predictor with rho = 0.5), with two keywords of later releases, chosen as for DPMSolverMultistepScheduler:
+      - final_sigmas_type, default "zero" (the last step lands on sigma = 0, x = m).  diffusers 0.27.2 has no such
+        keyword and always ends on the smallest training sigma, which final_sigmas_type="sigma_min" reproduces.
+      - rescale_betas_zero_snr, default True, the reference's setting; alpha_cumprod = 0 at the last training timestep
+        is replaced by 2^-24, as diffusers does.
+    One deliberate difference: diffusers' first-order predictor still adds -alpha_t B(h) * 0, which is NaN for bh1
+    onto a final sigma of 0 (B(h) = -inf); here that step is its limit, the data estimate m.
+    The timestep spacing and alpha_cumprod are DPMSolverMultistepScheduler's.  Its update is the
+    `hallo_b200_cfg_unipc_step` kernel; step() is the float64 host form, which the engine's loop does not call."""
+    order = 1
+    init_noise_sigma = 1.0
+
+    def __init__(self, num_train_timesteps: int = 1000, beta_start: float = 0.00085, beta_end: float = 0.012,
+                 beta_schedule: str = "linear", trained_betas=None, solver_order: int = 2,
+                 prediction_type: str = "v_prediction", thresholding: bool = False,
+                 dynamic_thresholding_ratio: float = 0.995, sample_max_value: float = 1.0, predict_x0: bool = True,
+                 solver_type: str = "bh2", lower_order_final: bool = True, disable_corrector: Sequence[int] = (),
+                 solver_p=None, use_karras_sigmas: bool = False, timestep_spacing: str = "trailing",
+                 steps_offset: int = 1, final_sigmas_type: str = "zero", rescale_betas_zero_snr: bool = True,
+                 **unused):
+        kw = dict(predict_x0=predict_x0, solver_order=solver_order, solver_type=solver_type, thresholding=thresholding,
+                  prediction_type=prediction_type, use_karras_sigmas=use_karras_sigmas, solver_p=solver_p, **unused)
+        _check_unipc_config(lambda k, d=None: kw.get(k, d))
+        if trained_betas is not None:
+            raise NotImplementedError("trained_betas: the engine's stand-ins build betas from beta_schedule")
+        if final_sigmas_type not in ("zero", "sigma_min"):
+            raise NotImplementedError(f"final_sigmas_type {final_sigmas_type!r}")
+        if final_sigmas_type == "zero" and not lower_order_final and solver_order == 2:
+            raise NotImplementedError("lower_order_final=False with final_sigmas_type='zero': a second-order UniPC "
+                                      "step onto sigma = 0 diverges; keep lower_order_final=True")
+        if timestep_spacing not in ("trailing", "leading", "linspace"):
+            raise NotImplementedError(f"timestep_spacing {timestep_spacing!r}")
+        self.alphas_cumprod = _solver_alphas_cumprod(num_train_timesteps, beta_start, beta_end, beta_schedule,
+                                                     rescale_betas_zero_snr)
+        self.num_train_timesteps = num_train_timesteps
+        self.solver_order, self.solver_type = int(solver_order), solver_type
+        self.lower_order_final = bool(lower_order_final)
+        self.disable_corrector = [int(k) for k in disable_corrector]
+        self.final_sigmas_type = final_sigmas_type
+        self.timestep_spacing, self.steps_offset = timestep_spacing, steps_offset
+        self.num_inference_steps: Optional[int] = None
+        self.timesteps = torch.arange(num_train_timesteps - 1, -1, -1)
+        self.sigmas = None
+        self._step_index: Optional[int] = None
+
+    def set_timesteps(self, num_inference_steps: int, device=None):
+        n = num_inference_steps
+        ts = _solver_timesteps(n, self.num_train_timesteps, self.timestep_spacing, self.steps_offset)
+        self.num_inference_steps = n
+        self.timesteps = torch.from_numpy(ts).to(device)
+        self._alpha, self._sigma = _solver_points(self.alphas_cumprod, ts, self.final_sigmas_type)
+        self.sigmas = torch.from_numpy(self._sigma / self._alpha).to(torch.float32)
+        with np.errstate(divide="ignore"):
+            self._lambda = np.log(self._alpha) - np.log(self._sigma)
+        self._step_index = None
+        self.model_outputs: List[Optional[torch.Tensor]] = [None] * self.solver_order
+        self.lower_order_nums = 0
+        self.last_sample: Optional[torch.Tensor] = None
+        self.this_order = 1
+
+    def scale_model_input(self, sample, timestep=None):
+        return sample
+
+    def _bh_update(self, a: int, b: int, x, m_a, m_k, k: Optional[int], model_t, rhos):
+        """diffusers' bh update from point a to point b in data prediction, float64:
+        x_b = (sigma_b / sigma_a) x - alpha_b h_phi_1 m_a - alpha_b B(h) (rho_0 D_1 [+ rho_t (model_t - m_a)]), with
+        D_1 = (m_k - m_a) / r_k from the earlier point k (order 2; k = None at order 1).  rhos = None solves diffusers'
+        system R rho = b (the order-2 corrector)."""
+        al, sg, lam = self._alpha, self._sigma, self._lambda
+        h = lam[b] - lam[a]
+        hh = -h
+        h_phi_1 = float(np.expm1(hh))
+        out = (sg[b] / sg[a]) * x - (al[b] * h_phi_1) * m_a
+        if k is None and model_t is None:
+            return out
+        bh = _unipc_bh(h, self.solver_type)
+        rks = ([(lam[k] - lam[a]) / h] if k is not None else []) + [1.0]
+        if rhos is None:
+            R, bv, h_phi_k, fact = [], [], h_phi_1 / hh - 1.0, 1
+            for j in range(1, len(rks) + 1):
+                R.append([r ** (j - 1) for r in rks])
+                bv.append(h_phi_k * fact / bh)
+                fact *= j + 1
+                h_phi_k = h_phi_k / hh - 1.0 / fact
+            rhos = np.linalg.solve(np.array(R), np.array(bv)).tolist()
+        res = torch.zeros_like(x)
+        if k is not None:
+            res = res + rhos[0] * ((m_k - m_a) / rks[0])
+        if model_t is not None:
+            res = res + rhos[-1] * (model_t - m_a)
+        return out - (al[b] * bh) * res
+
+    def step(self, model_output: torch.Tensor, timestep, sample: torch.Tensor, return_dict: bool = True):
+        """One UniPC step in diffusers' form, float64 on the host: the data estimate at the given sample, the corrector
+        (when i > 0 and i - 1 is not in disable_corrector) with the previous step's order, then the predictor.
+        Stateful like diffusers: the step index comes from the first timestep seen after set_timesteps; the data
+        estimates and the last corrected sample are kept between calls.  Returns the predicted next sample."""
+        if self.num_inference_steps is None:
+            raise ValueError("Number of inference steps is 'None', you need to run 'set_timesteps' after creating the scheduler")
+        if self._step_index is None:
+            self._step_index = self.timesteps.tolist().index(int(timestep))
+        i = self._step_index
+        x, v = sample.double(), model_output.double()
+        m = self._alpha[i] * x - self._sigma[i] * v                             # convert_model_output, at the UNet's input
+        if i > 0 and (i - 1) not in self.disable_corrector and self.last_sample is not None:
+            # multistep_uni_c_bh_update, from point i - 1 to i with the previous step's order: m_{i-1} is
+            # model_outputs[-1], m_{i-2} is model_outputs[-2]; rho = [0.5] at order 1, solve(R, b) at order 2
+            two = self.this_order == 2
+            x = self._bh_update(i - 1, i, self.last_sample, self.model_outputs[-1],
+                                self.model_outputs[-2] if two else None, i - 2 if two else None, m,
+                                None if two else [0.5])
+        self.model_outputs = self.model_outputs[1:] + [m]
+        n = len(self.timesteps)
+        this_order = min(self.solver_order, n - i) if self.lower_order_final else self.solver_order
+        self.this_order = min(this_order, self.lower_order_nums + 1)
+        self.last_sample = x
+        # multistep_uni_p_bh_update, from point i to i + 1: at order 2 diffusers fixes rho_p = [0.5]
+        two = self.this_order == 2
+        prev = self._bh_update(i, i + 1, x, m, self.model_outputs[-2] if two else None, i - 1 if two else None, None,
+                               [0.5])
+        if self.lower_order_nums < self.solver_order:
+            self.lower_order_nums += 1
+        self._step_index = i + 1
+        prev_sample = prev.to(sample.dtype)
+        if not return_dict:
+            return (prev_sample,)
+        return DDIMSchedulerOutput(prev_sample=prev_sample, pred_original_sample=m.to(sample.dtype))
+
+    def coef_table(self) -> torch.Tensor:
+        """[n_steps, 10] rows [alpha, sigma, kx, kL, k0, k1, k2, pc, p0, p1] for `hallo_b200_cfg_unipc_step` (see
+        unipc_table)."""
+        if self.num_inference_steps is None:
+            raise ValueError("run set_timesteps first")
+        return unipc_table(self._alpha, self._sigma, self.disable_corrector, self.solver_order, self.solver_type,
+                           self.lower_order_final)
+
+
 def latent_scales_of(sched) -> np.ndarray:
     """float64 [n + 1]: the factor between the scheduler's own latents and the engine's y at each step point, then the
     final point.  1 / alpha_i = sqrt(1 + sigma_i^2) for the Euler classes (x = y / alpha), ones for DDIM / DPM-Solver++
-    (whose latents are y).  The final scale is 1 for all of them."""
+    / UniPC (whose latents are y).  The final scale is 1 for all of them."""
     n = len(sched.timesteps)
     if type(sched).__name__ not in EULER_KINDS:
         return np.ones(n + 1)
@@ -499,8 +797,11 @@ def sampler_table_of(sched) -> Tuple[str, torch.Tensor]:
     thresholding / variance_type / prediction_type, timesteps, and its own sigmas = sigma / alpha, n + 1 of them) --
     ("multistep", [n, 5]) for EulerDiscreteScheduler and ("ancestral", [n, 5]) for EulerAncestralDiscreteScheduler,
     ours or diffusers' (recognised by class name, read through timesteps, sigmas and config.prediction_type /
-    use_karras_sigmas / interpolation_type / timestep_type / final_sigmas_type), and ("ddim", [n, 4]) from
-    coef_table_of for any other, DDIM-style, scheduler."""
+    use_karras_sigmas / interpolation_type / timestep_type / final_sigmas_type), ("unipc", [n, 10]) for
+    UniPCMultistepScheduler, ours or diffusers' (recognised by class name, read through timesteps, its own n + 1
+    sigmas and config.solver_order / solver_type / predict_x0 / lower_order_final / disable_corrector /
+    prediction_type / thresholding / use_karras_sigmas / solver_p), and ("ddim", [n, 4]) from coef_table_of for any
+    other, DDIM-style, scheduler."""
     if isinstance(sched, DPMSolverMultistepScheduler):
         return "multistep", sched.coef_table()
     cfg = getattr(sched, "config", None)
@@ -511,6 +812,13 @@ def sampler_table_of(sched) -> Tuple[str, torch.Tensor]:
         v = cfg.get(k, d) if isinstance(cfg, dict) else getattr(cfg, k, d)
         return d if v is None and d is not None else v
 
+    if type(sched).__name__ == "UniPCMultistepScheduler":               # before the DPM branch: it has solver_order too
+        if isinstance(sched, UniPCMultistepScheduler):
+            return "unipc", sched.coef_table()
+        _check_unipc_config(get)
+        al, sg = _points_from_sigmas(sched, "UniPC")
+        return "unipc", unipc_table(al, sg, get("disable_corrector", []) or [], int(get("solver_order", 2)),
+                                    get("solver_type", "bh2"), bool(get("lower_order_final", True)))
     euler = EULER_KINDS.get(type(sched).__name__)
     if euler is not None:
         _check_euler_config(get)
@@ -523,12 +831,7 @@ def sampler_table_of(sched) -> Tuple[str, torch.Tensor]:
         return "ddim", coef_table_of(sched)
     _check_dpm_config(get)
     n = len(sched.timesteps)
-    s = torch.as_tensor(sched.sigmas).detach().cpu().double().numpy()
-    if len(s) != n + 1:
-        raise ValueError(f"a {n}-step DPM-Solver++ schedule needs {n + 1} sigmas, got {len(s)}")
-    al = 1.0 / np.sqrt(1.0 + s * s)
-    with np.errstate(invalid="ignore"):
-        sg = np.where(np.isinf(s), 1.0, s * al)                   # sigma / alpha = inf: alpha = 0, sigma = 1
+    al, sg = _points_from_sigmas(sched, "DPM-Solver++")
     second = dpm_second_order_steps(n, int(get("solver_order")), bool(get("lower_order_final", True)),
                                     bool(get("euler_at_final", False)), get("final_sigmas_type", "zero"))
     return "multistep", dpm_solver_table(al, sg, second, get("solver_type", "midpoint"))

@@ -289,6 +289,15 @@ int hallo_b200_cfg_multistep_step(int dtype, const void* model_out, int64_t ldm,
 int hallo_b200_cfg_ancestral_step(int dtype, const void* model_out, int64_t ldm, float* latents, const void* noise,
                                   const float* coef, const int32_t* step, float guidance, int Cl, int F, int HW,
                                   hb_stream_t stream);
+/* CFG combine + UniPC (bh1 / bh2, order 1 or 2, data prediction) v-prediction update on fp32 latents [1, Cl, F, HW].
+ * coef: fp32 [n_steps, 10] = alpha, sigma, kx, kL, k0, k1, k2, pc, p0, p1; with v = v_u + guidance (v_c - v_u) and
+ * m = alpha x - sigma v (the data estimate at the sample the UNet saw), the corrector c = kx x + kL last_sample + k0 m
+ * + k1 x0_hist + k2 x0_hist2 (kx = 1, the rest 0 where it does not run), then x <- pc c + p0 m + p1 x0_hist,
+ * last_sample <- c, x0_hist2 <- x0_hist, x0_hist <- m.  last_sample, x0_hist, x0_hist2: fp32, shaped like latents; a
+ * term whose coefficient is 0 does not read its buffer, so step 0 of a schedule needs no initialised state. */
+int hallo_b200_cfg_unipc_step(int dtype, const void* model_out, int64_t ldm, float* latents, float* last_sample,
+                              float* x0_hist, float* x0_hist2, const float* coef, const int32_t* step, float guidance,
+                              int Cl, int F, int HW, hb_stream_t stream);
 int hallo_b200_advance_step(int32_t* step, int n_steps, hb_stream_t stream);
 /* channels-last [B*F*HW, ld] (first C columns) -> fp32 [B, C, F, HW] (the reference's output layout). */
 int hallo_b200_tokens_to_bcfhw(int dtype, const void* x, int64_t ld, float* out, int B, int C, int F, int HW,

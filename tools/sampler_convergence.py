@@ -1,13 +1,14 @@
-"""How accurately DDIM and DPM-Solver++ 2M integrate the denoising ODE at a given step count, and what a step costs.
+"""How accurately DDIM, DPM-Solver++ 2M and UniPC (bh2, order 2) integrate the denoising ODE at a given step count,
+and what a step costs.
 
 The workload is bench.py's: random-init weights (seed 0, drawn on the device), synthetic inputs (seed 42), one
 16-frame window at 512 x 512 (latent 64 x 64), CFG 3.5, fp16.  The reference solution is the mean of a 500-step DDIM
 run and a 500-step DPM-Solver++ 2M run; their mutual rel-L2 distance is printed as the floor below which no
 difference means anything.  Each row is the rel-L2 of the final latents against that reference and against the same
-sampler's 500-step run, and ms per step from CUDA events around the graph replays of that run.  A last line gives the
-sensitivity of the solution to its start: the rel-L2 change of 40-step DDIM's final latents when the initial latents
-move by 1e-3 (rel L2).  When that is large, this network's ODE amplifies any perturbation, discretisation error
-included, and step-count differences say little.  DDIM steps from t to t - 1000 // n (diffusers' rule), which
+sampler's 500-step run (UniPC has none: "-"), and ms per step from CUDA events around the graph replays of that
+run.  A last line gives the sensitivity of the solution to its start: the rel-L2 change of 40-step DDIM's final
+latents when the initial latents move by 1e-3 (rel L2).  When that is large, this network's ODE amplifies any
+perturbation, discretisation error included, and step-count differences say little.  DDIM steps from t to t - 1000 // n (diffusers' rule), which
 matches the trailing timesteps only when n divides 1000: at 400 steps each step covers 2 of the 2.5 timesteps between
 evaluations, so a 400-step DDIM run is not a converged solution (measured: 0.18 rel L2 from 400-step DPM-Solver++
 2M, against 2.7e-3 at 500 steps).  The card's name, power limit and the median SM clock sampled during the timed
@@ -16,7 +17,8 @@ replays are printed with the table.
 The weights are random-init, so this measures how accurately each sampler integrates this network's probability-flow
 ODE.  It says nothing about how videos from trained weights look: perceptual quality is not measured.
 
-    python tools/sampler_convergence.py [--ddim 10,20,25,40] [--dpm 10,15,20,25,40] [--ref-steps 500] [--json FILE]
+    python tools/sampler_convergence.py [--ddim 10,20,25,40] [--dpm 10,15,20,25,40] [--unipc 10,15,20,25]
+                                        [--ref-steps 500] [--json FILE]
 """
 from __future__ import annotations
 
@@ -47,6 +49,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--ddim", default="10,20,25,40")
     ap.add_argument("--dpm", default="10,15,20,25,40")
+    ap.add_argument("--unipc", default="10,15,20,25")
     ap.add_argument("--ref-steps", type=int, default=500,
                     help="reference step count; DDIM needs one that divides 1000")
     ap.add_argument("--size", type=int, default=64, help="latent side (64 = 512x512)")
@@ -59,7 +62,8 @@ def main():
     from bench import ClockSampler
     from hallo_b200.dist import window_inputs_to_device
     from hallo_b200.engine import DenoiseEngine, PackedWeights
-    from hallo_b200.scheduler import DDIMScheduler, DPMSolverMultistepScheduler, sampler_table_of
+    from hallo_b200.scheduler import (DDIMScheduler, DPMSolverMultistepScheduler, UniPCMultistepScheduler,
+                                      sampler_table_of)
     from hallo_b200.spec import UNetConfig
     from hallo_b200.synth import host_threads, synth_inputs, synth_state_dict_device
     torch.set_num_threads(host_threads())
@@ -89,7 +93,8 @@ def main():
         torch.cuda.synchronize()
         return eng.latents.clone(), e0.elapsed_time(e1) / n
 
-    samplers = {"DDIM": DDIMScheduler, "DPM-Solver++ 2M": DPMSolverMultistepScheduler}
+    samplers = {"DDIM": DDIMScheduler, "DPM-Solver++ 2M": DPMSolverMultistepScheduler,
+                "UniPC bh2": UniPCMultistepScheduler}
     clocks.start()
     ref_ddim, ms_ref_ddim = run(DDIMScheduler(), args.ref_steps)
     ref_dpm, ms_ref_dpm = run(DPMSolverMultistepScheduler(), args.ref_steps)
@@ -101,11 +106,12 @@ def main():
 
     floor = rel(ref_ddim, ref_dpm)
     rows = []
-    for name, steps in (("DDIM", args.ddim), ("DPM-Solver++ 2M", args.dpm)):
+    for name, steps in (("DDIM", args.ddim), ("DPM-Solver++ 2M", args.dpm), ("UniPC bh2", args.unipc)):
         for n in [int(s) for s in steps.split(",") if s]:
             lat, ms = run(samplers[name](), n)
             rows.append({"sampler": name, "steps": n, "rel_l2_vs_ref": rel(lat, ref),
-                         f"rel_l2_vs_own_{args.ref_steps}": rel(lat, own_ref[name]), "ms_per_step": ms,
+                         f"rel_l2_vs_own_{args.ref_steps}": rel(lat, own_ref[name]) if name in own_ref else None,
+                         "ms_per_step": ms,
                          "finite": bool(torch.isfinite(lat).all())})
     clk = clocks.stop()
     g = torch.Generator(device=dev).manual_seed(1)
@@ -125,7 +131,8 @@ def main():
     print(f"| sampler | steps | rel L2 vs reference | rel L2 vs same sampler at {args.ref_steps} | ms / step |")
     print("|---|---|---|---|---|")
     for r in rows:
-        print(f"| {r['sampler']} | {r['steps']} | {r['rel_l2_vs_ref']:.3e} | {r[f'rel_l2_vs_own_{args.ref_steps}']:.3e} "
+        own = r[f"rel_l2_vs_own_{args.ref_steps}"]
+        print(f"| {r['sampler']} | {r['steps']} | {r['rel_l2_vs_ref']:.3e} | {'-' if own is None else f'{own:.3e}'} "
               f"| {r['ms_per_step']:.1f} |")
     print(f"# sensitivity: 40-step DDIM final latents move by {sensitivity:.3e} rel L2 when the start moves by 1e-3")
     print(json.dumps(res))
