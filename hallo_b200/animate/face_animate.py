@@ -26,6 +26,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import vae_engine
+from ..engine import check_guidance_rescale
 from ..models.mutual_self_attention import ReferenceAttentionControl
 from ..scheduler import EULER_KINDS, latent_scales_of, sampler_table_of
 
@@ -198,7 +199,7 @@ class FaceAnimatePipeline:
                  generator=None, output_type: Optional[str] = "tensor", return_dict: bool = True,
                  callback: Optional[Callable[[int, int, torch.FloatTensor], None]] = None,
                  callback_steps: Optional[int] = 1, static: Optional[dict] = None,
-                 audio_guidance_scale: Optional[float] = None, **kwargs):
+                 audio_guidance_scale: Optional[float] = None, guidance_rescale: float = 0.0, **kwargs):
         """Denoise one window (face_animate.py:249-442) and decode it.
 
         guidance_scale s (> 1) is the classifier-free guidance weight.  audio_guidance_scale s_a, when given, weights
@@ -208,7 +209,16 @@ class FaceAnimatePipeline:
         so s moves identity / appearance fidelity and s_a moves lip motion.  s_a == s gives the two-branch guidance
         up to one rounding of v to the model dtype; each step runs about 1.5x the UNet rows.  None (the default) runs
         the two-branch path, unchanged.  Works with every supported scheduler, with callbacks and under
-        torch.distributed frame sharding."""
+        torch.distributed frame sharding.
+
+        guidance_rescale phi in [0, 1] (diffusers' `guidance_rescale`, Lin et al. 2023, arXiv:2305.08891, sec. 3.4)
+        counters the over-exposure CFG causes with the zero-terminal-SNR schedule these checkpoints use: each step's
+        guided v is rescaled towards the spread of the cond prediction v_c,
+            v = phi v std(v_c) / std(v) + (1 - phi) v,
+        with unbiased stds over the whole window (every channel, frame and pixel, across frame-sharded ranks).  With
+        audio_guidance_scale, v is the three-branch combine and v_c still the fully conditioned branch.  Where std(v)
+        is 0, v is kept as is (diffusers would give NaN).  0.0 (the default) runs exactly the path without it; a value
+        that is not finite or outside [0, 1] raises ValueError."""
         unet = self.denoising_unet
         device = self._execution_device
         height = height or unet.config.sample_size * self.vae_scale_factor
@@ -222,6 +232,7 @@ class FaceAnimatePipeline:
             audio_guidance_scale = float(audio_guidance_scale)
             if not math.isfinite(audio_guidance_scale):
                 raise ValueError(f"audio_guidance_scale must be finite, got {audio_guidance_scale}")
+        guidance_rescale = check_guidance_rescale(guidance_rescale)
         branches = 2 if audio_guidance_scale is None else 3
         self.scheduler.set_timesteps(num_inference_steps, device=device)
         timesteps = self.scheduler.timesteps
@@ -267,7 +278,8 @@ class FaceAnimatePipeline:
         eng.begin_window(encoder_hidden_states=ehs, audio_embedding=audio, mask_cond_fea=static["mask_cond"],
                          full_mask=static["full"], face_mask=static["face"], lip_mask=static["lip"],
                          motion_scale=motion_scale, banks=unet._banks)
-        eng.set_schedule(timesteps.tolist(), table, guidance_scale, sampler, audio_guidance=audio_guidance_scale)
+        eng.set_schedule(timesteps.tolist(), table, guidance_scale, sampler, audio_guidance=audio_guidance_scale,
+                         guidance_rescale=guidance_rescale)
         frames = list(eng.shard.frames)
         noise_rows = None
         if type(self.scheduler).__name__ in EULER_KINDS:

@@ -958,6 +958,119 @@ __global__ void cfg_guide3_kernel(T* __restrict__ model_out, long long ldm, floa
   }
 }
 
+// Guidance rescale (Lin et al. 2023, diffusers rescale_noise_cfg), in three kernels so the window-wide statistics stay
+// deterministic without atomics and can be shared across frame-sharded ranks:
+//   stats : v_cfg (the two- or three-branch combine above, fp32) per element; each of the HB_RESCALE_PARTIALS CTAs
+//           writes (sum v_c, sum v_c^2, sum v_cfg, sum v_cfg^2), accumulated in fp64, to partials[cta]
+//   reduce: one CTA sums the partials in fixed order and stores the 4 totals to every destination (this rank's slot
+//           of each rank's totals table)
+//   apply : every CTA forms k = phi std(v_c) / std(v_cfg) + (1 - phi) from the per-rank totals, summed in rank
+//           order, and writes [0 | k v_cfg] over halves 0 and 1 in the model dtype, ready for any cfg_*_step with
+//           guidance = 1 (as cfg_guide3_kernel does).  std is the unbiased one, over the n = ranks * Cl * F * HW
+//           elements of the window.
+// The grid of the stats kernel is fixed, the element-to-thread map depends on the shape alone, and every sum runs in
+// a fixed order: the same inputs give bitwise-equal factors on every run and on every rank.
+template <typename T>
+__device__ __forceinline__ float cfg_combine(const T* __restrict__ mo, long long ldm, int nb, float guidance,
+                                             float audio_guidance, long long total, long long i, int k, float& vc) {
+  const float vu = Cvt<T>::to_f(mo[i * ldm + k]);
+  vc = Cvt<T>::to_f(mo[(total + i) * ldm + k]);
+  if (nb == 3) {
+    const float vr = Cvt<T>::to_f(mo[(2 * total + i) * ldm + k]);
+    return vu + guidance * (vr - vu) + audio_guidance * (vc - vr);
+  }
+  return vu + guidance * (vc - vu);
+}
+
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+constexpr int kRescaleThreads = 256;
+
+template <typename T>
+__global__ void __launch_bounds__(kRescaleThreads) cfg_rescale_stats_kernel(
+    const T* __restrict__ model_out, long long ldm, int nb, float guidance, float audio_guidance, int Cl,
+    long long total, double* __restrict__ partials) {
+  pdl_wait();
+  pdl_launch();
+  double s[4] = {0.0, 0.0, 0.0, 0.0};
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    for (int k = 0; k < Cl; ++k) {
+      float vc;
+      const float v = cfg_combine(model_out, ldm, nb, guidance, audio_guidance, total, i, k, vc);
+      s[0] += vc;
+      s[1] += (double)vc * vc;                     // exact: a product of two floats fits a double
+      s[2] += v;
+      s[3] += (double)v * v;
+    }
+  }
+  __shared__ double red[4][kRescaleThreads / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const double w = warp_sum_d(s[q]);
+    if (lane == 0) red[q][warp] = w;
+  }
+  __syncthreads();
+  if (threadIdx.x < 4) {
+    double t = 0.0;
+    for (int w = 0; w < kRescaleThreads / 32; ++w) t += red[threadIdx.x][w];
+    partials[blockIdx.x * 4 + threadIdx.x] = t;
+  }
+}
+
+struct RescaleDst {
+  double* p[HB_MAX_PEERS];
+  int n;
+};
+
+// 4 warps: warp q sums quantity q over the partials (lane l takes l, l + 32, ...), then stores it to every destination.
+__global__ void __launch_bounds__(128) cfg_rescale_reduce_kernel(const double* __restrict__ partials, RescaleDst dst) {
+  pdl_wait();
+  pdl_launch();
+  const int q = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  double s = 0.0;
+  for (int j = lane; j < HB_RESCALE_PARTIALS; j += 32) s += partials[j * 4 + q];
+  s = warp_sum_d(s);
+  if (lane == 0)
+    for (int d = 0; d < dst.n; ++d) dst.p[d][q] = s;
+}
+
+template <typename T>
+__global__ void cfg_rescale_apply_kernel(T* __restrict__ model_out, long long ldm, int nb, float guidance,
+                                         float audio_guidance, float rescale, const double* __restrict__ totals,
+                                         int n_ranks, int Cl, long long total) {
+  pdl_wait();
+  pdl_launch();
+  __shared__ float factor;
+  if (threadIdx.x == 0) {
+    double s[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int r = 0; r < n_ranks; ++r)
+      for (int q = 0; q < 4; ++q) s[q] += totals[r * 4 + q];
+    const double n = (double)n_ranks * Cl * total;
+    double k = 1.0;
+    // one-pass variances; var(v_cfg) at or below the rounding of the fp64 sums counts as std = 0: v is kept as is
+    const double var_t = (s[1] - s[0] * s[0] / n) / (n - 1.0);
+    const double var_g = (s[3] - s[2] * s[2] / n) / (n - 1.0);
+    if (n > 1.0 && var_g > 1e-12 * (s[3] / n)) k = rescale * sqrt(fmax(var_t, 0.0) / var_g) + (1.0 - rescale);
+    factor = (float)k;
+  }
+  __syncthreads();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const float k = factor;
+  for (int c = 0; c < Cl; ++c) {
+    float vc;
+    const float v = cfg_combine(model_out, ldm, nb, guidance, audio_guidance, total, i, c, vc);
+    model_out[i * ldm + c] = Cvt<T>::from_f(0.f);
+    model_out[(total + i) * ldm + c] = Cvt<T>::from_f(k * v);
+  }
+}
+
 __global__ void advance_step_kernel(int* step, int n_steps) {
   pdl_wait();
   pdl_launch();
@@ -1359,6 +1472,60 @@ extern "C" int hallo_b200_cfg_guide3_step(int dtype, void* model_out, int64_t ld
   HB_DISPATCH_T(dtype, {
     launch_kernel(cfg_guide3_kernel<T>, (int)((total + 127) / 128), 128, 0, s, (T*)model_out, ldm, guidance,
                   audio_guidance, Cl, total);
+  })
+  HB_LAUNCH_CHECK();
+  return HB_OK;
+}
+
+static int check_rescale_args(const char* what, int dtype, int64_t ldm, int nb, int Cl, int F, int HW) {
+  if (dtype != HB_F16 && dtype != HB_BF16) return fail(HB_ERR_BAD_DTYPE, "%s: dtype %d", what, dtype);
+  if ((nb != 2 && nb != 3) || Cl < 1 || ldm < Cl || F < 1 || HW < 1)
+    return fail(HB_ERR_BAD_SHAPE, "%s: nb=%d Cl=%d ldm=%lld F=%d HW=%d", what, nb, Cl, (long long)ldm, F, HW);
+  return HB_OK;
+}
+
+extern "C" int hallo_b200_cfg_rescale_stats(int dtype, const void* model_out, int64_t ldm, int nb, float guidance,
+                                            float audio_guidance, int Cl, int F, int HW, double* partials,
+                                            hb_stream_t stream) {
+  if (!model_out || !partials) return fail(HB_ERR_NULL, "cfg_rescale_stats: null pointer");
+  if (int e = check_rescale_args("cfg_rescale_stats", dtype, ldm, nb, Cl, F, HW)) return e;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const long long total = (long long)F * HW;
+  HB_DISPATCH_T(dtype, {
+    launch_kernel(cfg_rescale_stats_kernel<T>, HB_RESCALE_PARTIALS, kRescaleThreads, 0, s, (const T*)model_out, ldm,
+                  nb, guidance, audio_guidance, Cl, total, partials);
+  })
+  HB_LAUNCH_CHECK();
+  return HB_OK;
+}
+
+extern "C" int hallo_b200_cfg_rescale_reduce(const double* partials, double* const* dst, int n_dst,
+                                             hb_stream_t stream) {
+  if (!partials || !dst) return fail(HB_ERR_NULL, "cfg_rescale_reduce: null pointer");
+  if (n_dst < 1 || n_dst > HB_MAX_PEERS) return fail(HB_ERR_BAD_SHAPE, "cfg_rescale_reduce: %d destinations", n_dst);
+  RescaleDst d{};
+  for (int i = 0; i < n_dst; ++i) {
+    if (!dst[i]) return fail(HB_ERR_NULL, "cfg_rescale_reduce: null destination %d", i);
+    d.p[i] = dst[i];
+  }
+  d.n = n_dst;
+  launch_kernel(cfg_rescale_reduce_kernel, 1, 128, 0, reinterpret_cast<cudaStream_t>(stream), partials, d);
+  HB_LAUNCH_CHECK();
+  return HB_OK;
+}
+
+extern "C" int hallo_b200_cfg_rescale_apply(int dtype, void* model_out, int64_t ldm, int nb, float guidance,
+                                            float audio_guidance, float rescale, const double* totals, int n_ranks,
+                                            int Cl, int F, int HW, hb_stream_t stream) {
+  if (!model_out || !totals) return fail(HB_ERR_NULL, "cfg_rescale_apply: null pointer");
+  if (int e = check_rescale_args("cfg_rescale_apply", dtype, ldm, nb, Cl, F, HW)) return e;
+  if (n_ranks < 1 || n_ranks > HB_MAX_PEERS || !(rescale >= 0.f && rescale <= 1.f))
+    return fail(HB_ERR_BAD_SHAPE, "cfg_rescale_apply: n_ranks=%d rescale=%g", n_ranks, (double)rescale);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const long long total = (long long)F * HW;
+  HB_DISPATCH_T(dtype, {
+    launch_kernel(cfg_rescale_apply_kernel<T>, (int)((total + 127) / 128), 128, 0, s, (T*)model_out, ldm, nb,
+                  guidance, audio_guidance, rescale, totals, n_ranks, Cl, total);
   })
   HB_LAUNCH_CHECK();
   return HB_OK;

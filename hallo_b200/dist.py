@@ -128,6 +128,7 @@ def sharded_vs_unsharded(eng, inp: dict, steps: int = 2, use_graph: bool = False
     ref.begin_window(**window_inputs_to_device(inp, eng.dev, eng.dtype))
     ref.n_steps, ref.guidance, ref.sampler = eng.n_steps, eng.guidance, eng.sampler
     ref.audio_guidance = eng.audio_guidance
+    ref.guidance_rescale = eng.guidance_rescale
     ref.t_table.copy_(eng.t_table)
     ref.coef.copy_(eng.coef)
     ref.coef_ms.copy_(eng.coef_ms)

@@ -19,6 +19,8 @@ from typing import List, Optional, Sequence
 
 import torch
 
+from .engine import check_guidance_rescale
+
 
 def process_audio_emb(audio_emb: torch.Tensor) -> torch.Tensor:
     """scripts/inference.py:95-114: frame i gets the embeddings of frames i-2..i+2 (indices clamped to the clip):
@@ -62,12 +64,15 @@ class ClipAnimator:
                  source_image_face_mask, source_image_lip_mask, audio_emb, audio_length: Optional[int] = None,
                  width: int = 512, height: int = 512, num_inference_steps: int = 40, guidance_scale: float = 3.5,
                  motion_scale: Sequence[float] = (1.0, 1.0, 1.0), generator=None, max_windows: Optional[int] = None,
-                 hoist: bool = True, audio_guidance_scale: Optional[float] = None) -> torch.Tensor:
+                 hoist: bool = True, audio_guidance_scale: Optional[float] = None,
+                 guidance_rescale: float = 0.0) -> torch.Tensor:
         """Arguments as scripts/inference.py prepares them: source_image_pixels (3, H, W) in [-1, 1], face region
         (3, H, W), face embedding (512,), three lists of 4 masks (1, L_l), audio_emb (S, 5, 12, 768) already through
         process_audio_emb, S a multiple of clip_length.  Returns the clip (3, audio_length, H, W) float32 on the host.
         audio_guidance_scale: a separate guidance weight for the audio (FaceAnimatePipeline.__call__); None keeps the
-        single guidance_scale."""
+        single guidance_scale.  guidance_rescale: phi in [0, 1] of guidance rescale (FaceAnimatePipeline.__call__),
+        checked before any work; 0.0 leaves the guided prediction as it is."""
+        guidance_rescale = check_guidance_rescale(guidance_rescale)
         pipe, cl = self.pipeline, self.clip_length
         dev = pipe.device
         src = source_image_pixels.unsqueeze(0).to(dev)
@@ -101,7 +106,8 @@ class ClipAnimator:
                        pixel_values_full_mask=full_m, pixel_values_face_mask=face_m, pixel_values_lip_mask=lip_m,
                        width=width, height=height, video_length=cl, num_inference_steps=num_inference_steps,
                        guidance_scale=guidance_scale, generator=generator, motion_scale=list(motion_scale),
-                       static=static, output_type="device", audio_guidance_scale=audio_guidance_scale)
+                       static=static, output_type="device", audio_guidance_scale=audio_guidance_scale,
+                       guidance_rescale=guidance_rescale)
             previous = out.videos                                                  # (1, 3, cl, H, W) on the device
             done = torch.cuda.Event()
             done.record()

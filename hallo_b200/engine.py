@@ -50,6 +50,14 @@ class Shard:
                                             # local ones, so the numbers it produces are not a valid denoising result
 
 
+def check_guidance_rescale(guidance_rescale) -> float:
+    """phi of guidance rescale as a float; ValueError unless finite and in [0, 1]."""
+    phi = float(guidance_rescale)
+    if not (math.isfinite(phi) and 0.0 <= phi <= 1.0):
+        raise ValueError(f"guidance_rescale must be a finite number in [0, 1], got {guidance_rescale}")
+    return phi + 0.0                     # -0.0 -> 0.0
+
+
 class PackedWeights:
     """Device-resident, kernel-ready copies of the state dict (packed once per model load)."""
     kind = "3d"        # refnet.ReferenceNetWeights sets "2d": resnets + spatial blocks only, no output head
@@ -225,7 +233,8 @@ class DenoiseEngine:
         self.n_steps = 1
         self.guidance = 1.0
         self.audio_guidance: Optional[float] = None      # three-branch engines (halves 0, 1, 2) only
-        # (n_steps, guidance, sampler, audio_guidance) baked into the graph: kernel arguments / choice
+        self.guidance_rescale = 0.0                      # phi of guidance rescale; 0 issues no rescale kernels
+        # (n_steps, guidance, sampler, guidance_rescale, audio_guidance) baked into the graph: kernel arguments / choice
         self._captured_with = None
         assert self.nm + n_frames <= self.cfg.pe_max_len, "temporal length exceeds the positional-encoding table"
         self.latents = torch.zeros(1, self.cfg.in_channels, self.fl, h, w, dtype=torch.float32, device=self.dev)
@@ -266,6 +275,8 @@ class DenoiseEngine:
             regions.append((f"x18.{name}", nb * (nm + f) * (L // R) * C * esz))
             recv = max(recv, nb * fl * L * C * esz)
         regions.append(("recv", recv))
+        # guidance rescale: every rank's 4 fp64 window sums, slot r written by rank r (see _cfg_rescale)
+        regions.append(("rescale", R * 4 * 8))
         self.me = sh.rank_in_group
         if sh.group_size > 1 and sh.exchange == "peer":
             from .peer import PeerArena
@@ -445,7 +456,8 @@ class DenoiseEngine:
         torch.cuda.current_stream().synchronize()
 
     def set_schedule(self, timesteps: Sequence[int], coef: torch.Tensor, guidance: float, sampler: str = "ddim",
-                     noise: Optional[torch.Tensor] = None, audio_guidance: Optional[float] = None):
+                     noise: Optional[torch.Tensor] = None, audio_guidance: Optional[float] = None,
+                     guidance_rescale: float = 0.0):
         """Per-window schedule.  The tables keep their device addresses (a captured graph reads them); the step count
         and the guidance scale are kernel ARGUMENTS of the captured launches and the sampler chooses the step kernel,
         so changing any of them drops the graph.  sampler "ddim": coef is the [n, 4] DDIM table
@@ -456,7 +468,10 @@ class DenoiseEngine:
         corrector and is first order, so a new window needs no reset of last_sample or the history either.
         audio_guidance: the audio scale s_a of a three-branch engine (shard halves (0, 1, 2)), which combines
         v = v_u + guidance (v_r - v_u) + s_a (v_c - v_r); required there and refused by a two-branch engine.  It is a
-        kernel argument of the captured graph too."""
+        kernel argument of the captured graph too.
+        guidance_rescale: phi in [0, 1] of guidance rescale (diffusers rescale_noise_cfg): the combined v is rescaled
+        towards the window-wide std of v_c, v = phi v std(v_c) / std(v) + (1 - phi) v.  0 (the default) runs no extra
+        kernel; any other value is part of the captured graph as well."""
         n = len(timesteps)
         if n > self.MAX_STEPS:
             raise ValueError(f"{n} inference steps exceed the engine's schedule capacity ({self.MAX_STEPS})")
@@ -472,6 +487,7 @@ class DenoiseEngine:
                              f"two-branch one; this engine has halves {tuple(self.shard.halves)}")
         if audio_guidance is not None and not math.isfinite(audio_guidance):
             raise ValueError(f"audio_guidance must be finite, got {audio_guidance}")
+        guidance_rescale = check_guidance_rescale(guidance_rescale)
         self.n_steps = n
         self.t_table[:n].copy_(torch.tensor([float(t) for t in timesteps], dtype=torch.float32))
         table = {"ddim": self.coef, "unipc": self.coef_uni}.get(sampler, self.coef_ms)
@@ -479,6 +495,7 @@ class DenoiseEngine:
         self.sampler = sampler
         self.guidance = float(guidance)
         self.audio_guidance = None if audio_guidance is None else float(audio_guidance)
+        self.guidance_rescale = guidance_rescale
         if self.graph is not None and self._captured_with != self._schedule_key():
             self.graph = None
         self.step_idx.zero_()
@@ -486,7 +503,8 @@ class DenoiseEngine:
             self.set_noise(noise)
 
     def _schedule_key(self):
-        return (self.n_steps, self.guidance, self.sampler, self.audio_guidance)
+        # the audio scale stays the last element
+        return (self.n_steps, self.guidance, self.sampler, self.guidance_rescale, self.audio_guidance)
 
     def set_noise(self, noise: torch.Tensor, step: Optional[int] = None):
         """Ancestral sampler: copy this window's per-step Gaussian draws, [n_steps, Cl, fl, h, w] (this rank's frames,
@@ -829,13 +847,16 @@ class DenoiseEngine:
     @torch.no_grad()
     def _step_tail(self):
         """CFG combine + scheduler update (DDIM, DPM-Solver++ / Euler, Euler-a or UniPC) + step counter
-        (face_animate.py:415-420).  Three branches: the combine writes [0 | v] over the first two halves, and the
-        sampler's kernel then runs with guidance 1, which passes v through exactly."""
+        (face_animate.py:415-420).  Three branches or guidance rescale: a pre-pass writes the combined v as [0 | v] over
+        the first two halves, and the sampler's kernel then runs with guidance 1, which passes v through exactly."""
         mo = self.model_out                    # every CFG half of the local frames: the combine is rank-local
         guidance = self.guidance
-        if self.nb == 3:
-            if self.audio_guidance is None:
-                raise RuntimeError("a three-branch engine needs set_schedule(..., audio_guidance=) before it steps")
+        if self.nb == 3 and self.audio_guidance is None:
+            raise RuntimeError("a three-branch engine needs set_schedule(..., audio_guidance=) before it steps")
+        if self.guidance_rescale > 0.0:
+            self._cfg_rescale(mo)
+            guidance = 1.0
+        elif self.nb == 3:
             ops.cfg_guide3_step(mo, cl=self.cfg.in_channels, frames=self.fl, hw=self.h * self.w,
                                 guidance=self.guidance, audio_guidance=self.audio_guidance)
             guidance = 1.0
@@ -851,6 +872,34 @@ class DenoiseEngine:
         else:
             ops.cfg_ddim_step(mo, self.latents, self.coef, self.step_idx, guidance=guidance)
         ops.advance_step(self.step_idx, self.n_steps)
+
+    def _cfg_rescale(self, mo):
+        """Guidance rescale over the whole window: this rank's fp64 sums (stats + reduce), every rank's sums on every
+        rank in rank order, then [0 | v] with the rescaled v (apply).  Each rank reduces all R totals itself, in the
+        same order, so all ranks apply a bitwise-identical factor."""
+        sh, R = self.shard, self.R
+        me = sh.rank_in_group
+        kw = dict(nb=self.nb, cl=self.cfg.in_channels, frames=self.fl, hw=self.h * self.w, guidance=self.guidance,
+                  audio_guidance=self.audio_guidance or 0.0)
+        part = self.buf("rescale.partials", ops.RESCALE_PARTIALS, 4, torch.float64)
+        ops.cfg_rescale_stats(mo, part, **kw)
+        if self.arena is not None:
+            # rank me stores its sums into slot me of every rank's table.  A slot is rewritten only one step later,
+            # after the motion modules' barriers of that step, by which time its reader has consumed it.
+            totals = self.arena.local("rescale", (R, 4), torch.float64)
+            ops.cfg_rescale_reduce(part, self.arena.addrs("rescale", me * 4 * 8))
+            self.arena.barrier()
+        elif sh.group_size > 1:
+            import torch.distributed as dist
+            send = self.buf("rescale.send", R, 4, torch.float64)
+            totals = self.buf("rescale.totals", R, 4, torch.float64)
+            ops.cfg_rescale_reduce(part, list(send))                   # the same 4 sums for every rank
+            dist.all_to_all_single(totals, send, group=sh.group)        # row s = rank s's sums
+        else:
+            # R = 1, or emulate_group: the emulated peers' sums are copies of this rank's
+            totals = self.buf("rescale.totals", R, 4, torch.float64)
+            ops.cfg_rescale_reduce(part, list(totals))
+        ops.cfg_rescale_apply(mo, totals, rescale=self.guidance_rescale, **kw)
 
     # ------------------------------------------------------------------ public
     @torch.no_grad()

@@ -491,6 +491,55 @@ def cfg_guide3_step(model_out: torch.Tensor, *, cl: int, frames: int, hw: int, g
     return model_out
 
 
+RESCALE_PARTIALS = 256          # HB_RESCALE_PARTIALS: rows of cfg_rescale_stats' partials workspace
+
+
+@_timed(lambda *a, **kw: "cfg_rescale_stats")
+def cfg_rescale_stats(model_out: torch.Tensor, partials: torch.Tensor, *, nb: int, cl: int, frames: int, hw: int,
+                      guidance: float, audio_guidance: float = 0.0) -> torch.Tensor:
+    """Guidance rescale, statistics: model_out [nb*frames*hw, ld] tokens (nb = 2: uncond, cond; 3: also cond with zero
+    audio); partials: fp64 [RESCALE_PARTIALS, 4] <- per-CTA sums of v_c, v_c^2, v_cfg, v_cfg^2, with v_cfg the CFG
+    combine of cfg_*_step (nb = 2) or cfg_guide3_step (nb = 3)."""
+    assert model_out.shape[0] >= nb * frames * hw
+    assert partials.dtype == torch.float64 and partials.is_contiguous() and partials.numel() >= RESCALE_PARTIALS * 4
+    lib.check(lib.load().hallo_b200_cfg_rescale_stats(
+        _i(lib.dtype_code(model_out.dtype)), C.c_void_p(lib.ptr(model_out)), C.c_int64(_rowmajor_ld(model_out)), _i(nb),
+        C.c_float(guidance), C.c_float(audio_guidance), _i(cl), _i(frames), _i(hw), C.c_void_p(lib.ptr(partials)),
+        lib.current_stream()), "cfg_rescale_stats")
+    return partials
+
+
+@_timed(lambda *a, **kw: "cfg_rescale_reduce")
+def cfg_rescale_reduce(partials: torch.Tensor, dst) -> None:
+    """Guidance rescale, reduction: the 4 totals of `partials` stored to every destination of `dst`, a list of fp64
+    [4] tensors or device addresses (peer memory: this rank's slot in each rank's totals table)."""
+    assert partials.dtype == torch.float64 and partials.is_contiguous() and 1 <= len(dst)
+    addrs = []
+    for d in dst:
+        if isinstance(d, torch.Tensor):
+            assert d.dtype == torch.float64 and d.is_contiguous() and d.numel() == 4
+            d = lib.ptr(d)
+        addrs.append(C.c_void_p(int(d)))
+    arr = (C.c_void_p * len(addrs))(*addrs)
+    lib.check(lib.load().hallo_b200_cfg_rescale_reduce(C.c_void_p(lib.ptr(partials)), arr, _i(len(addrs)),
+                                                       lib.current_stream()), "cfg_rescale_reduce")
+
+
+@_timed(lambda *a, **kw: "cfg_rescale_apply")
+def cfg_rescale_apply(model_out: torch.Tensor, totals: torch.Tensor, *, nb: int, cl: int, frames: int, hw: int,
+                      guidance: float, audio_guidance: float = 0.0, rescale: float) -> torch.Tensor:
+    """Guidance rescale, in place: totals fp64 [ranks, 4] (every rank's sums, in rank order) give
+    v = rescale v_cfg std(v_c) / std(v_cfg) + (1 - rescale) v_cfg over the whole window, written back as [0 | v] over
+    the first two halves, ready for any cfg_*_step with guidance = 1."""
+    assert model_out.shape[0] >= nb * frames * hw
+    assert totals.dtype == torch.float64 and totals.is_contiguous() and totals.dim() == 2 and totals.shape[1] == 4
+    lib.check(lib.load().hallo_b200_cfg_rescale_apply(
+        _i(lib.dtype_code(model_out.dtype)), C.c_void_p(lib.ptr(model_out)), C.c_int64(_rowmajor_ld(model_out)), _i(nb),
+        C.c_float(guidance), C.c_float(audio_guidance), C.c_float(rescale), C.c_void_p(lib.ptr(totals)),
+        _i(totals.shape[0]), _i(cl), _i(frames), _i(hw), lib.current_stream()), "cfg_rescale_apply")
+    return model_out
+
+
 def advance_step(step: torch.Tensor, n_steps: int) -> None:
     lib.check(lib.load().hallo_b200_advance_step(C.c_void_p(lib.ptr(step)), _i(n_steps), lib.current_stream()),
               "advance_step")

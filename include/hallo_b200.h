@@ -305,6 +305,29 @@ int hallo_b200_cfg_unipc_step(int dtype, const void* model_out, int64_t ldm, flo
  * guidance = 1.  With audio_guidance == guidance this is the two-branch combine up to that one rounding. */
 int hallo_b200_cfg_guide3_step(int dtype, void* model_out, int64_t ldm, float guidance, float audio_guidance, int Cl,
                                int F, int HW, hb_stream_t stream);
+/* Guidance rescale (diffusers rescale_noise_cfg) over a whole window, possibly frame-sharded over ranks, in three
+ * stream-ordered calls on model_out [nb*F*HW, ldm] (nb = 2: rows uncond, cond; nb = 3: uncond, cond, cond with zero
+ * audio tokens; first Cl columns valid).  v_cfg is the fp32 combine of cfg_*_step (nb = 2) or cfg_guide3_step
+ * (nb = 3) with the same guidance / audio_guidance; the "text" prediction is always the cond rows, v_c.
+ *   stats : partials [HB_RESCALE_PARTIALS, 4] fp64 <- per-CTA (sum v_c, sum v_c^2, sum v_cfg, sum v_cfg^2) of this
+ *           rank's elements.
+ *   reduce: the 4 totals of the partials (summed in a fixed order) are stored to each of dst[0 .. n_dst) (host array
+ *           of device pointers: this rank's slot in every rank's totals table, or copies).
+ *   apply : totals [n_ranks, 4] fp64, summed in rank order, over n = n_ranks*Cl*F*HW elements (every rank holds F
+ *           frames) give the unbiased std_t = std(v_c) and std_g = std(v_cfg), and
+ *             v = rescale * v_cfg * std_t / std_g + (1 - rescale) * v_cfg,
+ *           written as 0 over the uncond rows and v (rounded to the model dtype) over the cond rows, so any cfg_*_step
+ *           then applies the scheduler update to v with guidance = 1.  Where std_g is 0 (up to the rounding of the
+ *           fp64 sums, var(v_cfg) <= 1e-12 mean(v_cfg^2)) v = v_cfg is written instead of NaN.  rescale in [0, 1].
+ * No atomics: equal inputs give bitwise-equal outputs, and ranks holding equal totals apply the same factor. */
+#define HB_RESCALE_PARTIALS 256
+int hallo_b200_cfg_rescale_stats(int dtype, const void* model_out, int64_t ldm, int nb, float guidance,
+                                 float audio_guidance, int Cl, int F, int HW, double* partials, hb_stream_t stream);
+int hallo_b200_cfg_rescale_reduce(const double* partials, double* const* dst /* host array */, int n_dst,
+                                  hb_stream_t stream);
+int hallo_b200_cfg_rescale_apply(int dtype, void* model_out, int64_t ldm, int nb, float guidance, float audio_guidance,
+                                 float rescale, const double* totals, int n_ranks, int Cl, int F, int HW,
+                                 hb_stream_t stream);
 int hallo_b200_advance_step(int32_t* step, int n_steps, hb_stream_t stream);
 /* channels-last [B*F*HW, ld] (first C columns) -> fp32 [B, C, F, HW] (the reference's output layout). */
 int hallo_b200_tokens_to_bcfhw(int dtype, const void* x, int64_t ld, float* out, int B, int C, int F, int HW,
