@@ -9,7 +9,7 @@ What changed is who runs the 40-step loop (:384-427): instead of 40 x {torch.cat
 scheduler.step} this hands the window to hallo_b200.engine.DenoiseEngine, which replays one captured CUDA
 graph per step (UNet3D forward + CFG combine + DDIM, DPM-Solver++, Euler, Euler-a or UniPC update, all sm_90a kernels).
 With `audio_guidance_scale` the window runs a third CFG branch (the cond inputs with zero audio) so lip motion gets a
-guidance weight of its own.
+guidance weight of its own.  With `guidance_interval` the steps outside the interval run the cond rows alone.
 Euler-a's per-step noise is drawn on the host from `generator` in the reference's order (initial latents, then one
 draw per step) and uploaded once per window into the engine's noise table.  The VAE's encode / decode run on
 hallo_b200.vae_engine (sm_90a kernels as well) when `vae` is an SD-1.5 AutoencoderKL on CUDA in fp16 / bf16, and
@@ -19,14 +19,14 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import Callable, List, Optional, Union
+from typing import Callable, List, Optional, Tuple, Union
 
 import numpy as np
 import torch
 import torch.nn.functional as F
 
 from .. import vae_engine
-from ..engine import check_guidance_rescale
+from ..engine import check_guidance_interval, check_guidance_rescale, guided_steps
 from ..models.mutual_self_attention import ReferenceAttentionControl
 from ..scheduler import EULER_KINDS, latent_scales_of, sampler_table_of
 
@@ -199,7 +199,8 @@ class FaceAnimatePipeline:
                  generator=None, output_type: Optional[str] = "tensor", return_dict: bool = True,
                  callback: Optional[Callable[[int, int, torch.FloatTensor], None]] = None,
                  callback_steps: Optional[int] = 1, static: Optional[dict] = None,
-                 audio_guidance_scale: Optional[float] = None, guidance_rescale: float = 0.0, **kwargs):
+                 audio_guidance_scale: Optional[float] = None, guidance_rescale: float = 0.0,
+                 guidance_interval: Optional[Tuple[float, float]] = None, **kwargs):
         """Denoise one window (face_animate.py:249-442) and decode it.
 
         guidance_scale s (> 1) is the classifier-free guidance weight.  audio_guidance_scale s_a, when given, weights
@@ -218,7 +219,15 @@ class FaceAnimatePipeline:
         with unbiased stds over the whole window (every channel, frame and pixel, across frame-sharded ranks).  With
         audio_guidance_scale, v is the three-branch combine and v_c still the fully conditioned branch.  Where std(v)
         is 0, v is kept as is (diffusers would give NaN).  0.0 (the default) runs exactly the path without it; a value
-        that is not finite or outside [0, 1] raises ValueError."""
+        that is not finite or outside [0, 1] raises ValueError.
+
+        guidance_interval (t_lo, t_hi) limits guidance to an interval of noise levels (Kynkaanniemi et al. 2024,
+        arXiv:2404.07724), in the scheduler's own timestep units (the values of scheduler.timesteps, floats for the
+        Euler classes): step i is guided iff t_lo <= timesteps[i] <= t_hi.  An unguided step runs the UNet on the cond
+        branch alone (half the rows of a two-branch step, a third of a three-branch one) and steps on v = v_c; guidance
+        rescale and the audio scale apply to guided steps only.  Sampler state carries across guided and unguided
+        steps.  None (the default) guides every step, unchanged; an interval that holds no step runs the whole window
+        unguided.  A value that is not a pair of finite numbers with t_lo <= t_hi raises ValueError."""
         unet = self.denoising_unet
         device = self._execution_device
         height = height or unet.config.sample_size * self.vae_scale_factor
@@ -233,6 +242,7 @@ class FaceAnimatePipeline:
             if not math.isfinite(audio_guidance_scale):
                 raise ValueError(f"audio_guidance_scale must be finite, got {audio_guidance_scale}")
         guidance_rescale = check_guidance_rescale(guidance_rescale)
+        guidance_interval = check_guidance_interval(guidance_interval)
         branches = 2 if audio_guidance_scale is None else 3
         self.scheduler.set_timesteps(num_inference_steps, device=device)
         timesteps = self.scheduler.timesteps
@@ -279,7 +289,7 @@ class FaceAnimatePipeline:
                          full_mask=static["full"], face_mask=static["face"], lip_mask=static["lip"],
                          motion_scale=motion_scale, banks=unet._banks)
         eng.set_schedule(timesteps.tolist(), table, guidance_scale, sampler, audio_guidance=audio_guidance_scale,
-                         guidance_rescale=guidance_rescale)
+                         guidance_rescale=guidance_rescale, guided=guided_steps(timesteps.tolist(), guidance_interval))
         frames = list(eng.shard.frames)
         noise_rows = None
         if type(self.scheduler).__name__ in EULER_KINDS:
@@ -307,8 +317,12 @@ class FaceAnimatePipeline:
             eng.latents.copy_(latents[:, :, frames].float())
         else:
             eng.latents.copy_((latents[:, :, frames].double() / scales[0]).float())
-        if self.use_cuda_graph and callback is None and eng.graph is None:
-            eng.capture()
+        if self.use_cuda_graph and callback is None:
+            if eng.graph is None:
+                eng.capture()
+            cond = eng.cond_engine()                 # the unguided steps' engine, when the interval leaves any out
+            if cond is not None and cond.graph is None:
+                cond.capture()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i, t in enumerate(timesteps):

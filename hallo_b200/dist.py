@@ -104,14 +104,19 @@ def sharded_vs_unsharded(eng, inp: dict, steps: int = 2, use_graph: bool = False
     rank, world = sh.rank_in_group, sh.group_size
     lat0 = inp["sample"][:1].float()
     eng.latents.copy_(lat0[:, :, list(sh.frames)].to(eng.dev))
-    eng.step_idx.zero_()
-    saved = eng.graph
+    eng.reset_steps()
+    cond = eng.cond_engine()                                              # guidance interval: the unguided steps' engine
+    saved = eng.graph, None if cond is None else cond.graph
     if not use_graph:
         eng.graph = None
+        if cond is not None:
+            cond.graph = None
     for _ in range(steps):
         eng.step()
     torch.cuda.synchronize()
-    eng.graph = saved
+    eng.graph = saved[0]
+    if cond is not None:
+        cond.graph = saved[1]
     parts = [torch.empty_like(eng.latents) for _ in range(world)]
     dist.all_gather(parts, eng.latents.contiguous(), group=sh.group)
     noise = None
@@ -119,7 +124,7 @@ def sharded_vs_unsharded(eng, inp: dict, steps: int = 2, use_graph: bool = False
         nparts = [torch.empty_like(eng.noise) for _ in range(world)]
         dist.all_gather(nparts, eng.noise, group=sh.group)
         noise = torch.cat(nparts, dim=2)
-    eng.step_idx.zero_()
+    eng.reset_steps()
     if rank != 0:
         dist.barrier(group=sh.group)
         return None
@@ -129,6 +134,7 @@ def sharded_vs_unsharded(eng, inp: dict, steps: int = 2, use_graph: bool = False
     ref.n_steps, ref.guidance, ref.sampler = eng.n_steps, eng.guidance, eng.sampler
     ref.audio_guidance = eng.audio_guidance
     ref.guidance_rescale = eng.guidance_rescale
+    ref.guided = eng.guided
     ref.t_table.copy_(eng.t_table)
     ref.coef.copy_(eng.coef)
     ref.coef_ms.copy_(eng.coef_ms)
@@ -140,6 +146,7 @@ def sharded_vs_unsharded(eng, inp: dict, steps: int = 2, use_graph: bool = False
         ref.step()
     torch.cuda.synchronize()
     err = float((full - ref.latents).norm() / ref.latents.norm())
+    ref.release()
     del ref
     torch.cuda.empty_cache()
     dist.barrier(group=sh.group)

@@ -15,11 +15,11 @@ windows are strictly sequential (motion-frame dependency).  What this driver cha
 from __future__ import annotations
 
 import math
-from typing import List, Optional, Sequence
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
-from .engine import check_guidance_rescale
+from .engine import check_guidance_interval, check_guidance_rescale
 
 
 def process_audio_emb(audio_emb: torch.Tensor) -> torch.Tensor:
@@ -65,14 +65,18 @@ class ClipAnimator:
                  width: int = 512, height: int = 512, num_inference_steps: int = 40, guidance_scale: float = 3.5,
                  motion_scale: Sequence[float] = (1.0, 1.0, 1.0), generator=None, max_windows: Optional[int] = None,
                  hoist: bool = True, audio_guidance_scale: Optional[float] = None,
-                 guidance_rescale: float = 0.0) -> torch.Tensor:
+                 guidance_rescale: float = 0.0,
+                 guidance_interval: Optional[Tuple[float, float]] = None) -> torch.Tensor:
         """Arguments as scripts/inference.py prepares them: source_image_pixels (3, H, W) in [-1, 1], face region
         (3, H, W), face embedding (512,), three lists of 4 masks (1, L_l), audio_emb (S, 5, 12, 768) already through
         process_audio_emb, S a multiple of clip_length.  Returns the clip (3, audio_length, H, W) float32 on the host.
         audio_guidance_scale: a separate guidance weight for the audio (FaceAnimatePipeline.__call__); None keeps the
         single guidance_scale.  guidance_rescale: phi in [0, 1] of guidance rescale (FaceAnimatePipeline.__call__),
-        checked before any work; 0.0 leaves the guided prediction as it is."""
+        checked before any work; 0.0 leaves the guided prediction as it is.  guidance_interval: (t_lo, t_hi) in the
+        scheduler's timestep units; steps outside it run unguided on the cond branch alone
+        (FaceAnimatePipeline.__call__), checked before any work; None guides every step."""
         guidance_rescale = check_guidance_rescale(guidance_rescale)
+        guidance_interval = check_guidance_interval(guidance_interval)
         pipe, cl = self.pipeline, self.clip_length
         dev = pipe.device
         src = source_image_pixels.unsqueeze(0).to(dev)
@@ -107,7 +111,7 @@ class ClipAnimator:
                        width=width, height=height, video_length=cl, num_inference_steps=num_inference_steps,
                        guidance_scale=guidance_scale, generator=generator, motion_scale=list(motion_scale),
                        static=static, output_type="device", audio_guidance_scale=audio_guidance_scale,
-                       guidance_rescale=guidance_rescale)
+                       guidance_rescale=guidance_rescale, guidance_interval=guidance_interval)
             previous = out.videos                                                  # (1, 3, cl, H, W) on the device
             done = torch.cuda.Event()
             done.record()

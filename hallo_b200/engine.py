@@ -25,7 +25,7 @@ the collectives (hallo_b200/peer.py); an NCCL all-to-all variant of the same exc
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -56,6 +56,30 @@ def check_guidance_rescale(guidance_rescale) -> float:
     if not (math.isfinite(phi) and 0.0 <= phi <= 1.0):
         raise ValueError(f"guidance_rescale must be a finite number in [0, 1], got {guidance_rescale}")
     return phi + 0.0                     # -0.0 -> 0.0
+
+
+def check_guidance_interval(guidance_interval) -> Optional[Tuple[float, float]]:
+    """(t_lo, t_hi) of guidance limited to an interval as floats, or None; ValueError unless a pair of finite numbers
+    with t_lo <= t_hi."""
+    if guidance_interval is None:
+        return None
+    try:
+        lo, hi = guidance_interval
+        lo, hi = float(lo), float(hi)
+    except (TypeError, ValueError):
+        raise ValueError(f"guidance_interval must be a pair (t_lo, t_hi) of numbers, got {guidance_interval!r}") from None
+    if not (math.isfinite(lo) and math.isfinite(hi)) or lo > hi:
+        raise ValueError(f"guidance_interval must be finite with t_lo <= t_hi, got {guidance_interval!r}")
+    return lo, hi
+
+
+def guided_steps(timesteps: Sequence, guidance_interval) -> Optional[List[bool]]:
+    """Per-step mask of guidance limited to an interval: step i is guided iff t_lo <= timesteps[i] <= t_hi (the
+    scheduler's own timestep values, closed ends).  None for no interval: every step is guided."""
+    iv = check_guidance_interval(guidance_interval)
+    if iv is None:
+        return None
+    return [iv[0] <= float(t) <= iv[1] for t in timesteps]
 
 
 class PackedWeights:
@@ -236,19 +260,31 @@ class DenoiseEngine:
         self.guidance_rescale = 0.0                      # phi of guidance rescale; 0 issues no rescale kernels
         # (n_steps, guidance, sampler, guidance_rescale, audio_guidance) baked into the graph: kernel arguments / choice
         self._captured_with = None
+        # guidance limited to an interval: per-step mask (None: every step guided) and the cond-only companion that runs
+        # the unguided steps (see cond_engine); the host-side step counter picks which of the two graphs a step replays
+        self.guided: Optional[Tuple[bool, ...]] = None
+        self._cond: Optional["DenoiseEngine"] = None
+        self._next_step = 0
+        self._window_args: Optional[dict] = None        # the last begin_window's inputs, for the companion's window
+        self._window_gen = 0
         assert self.nm + n_frames <= self.cfg.pe_max_len, "temporal length exceeds the positional-encoding table"
         self.latents = torch.zeros(1, self.cfg.in_channels, self.fl, h, w, dtype=torch.float32, device=self.dev)
         self.x0_hist = torch.zeros_like(self.latents)
         self.last_sample = torch.zeros_like(self.latents)      # UniPC: the previous step's corrected sample
         self.x0_hist2 = torch.zeros_like(self.latents)         # UniPC: the data estimate of two steps back
         self.model_out: Optional[torch.Tensor] = None
+        if self.nb == 1:
+            # cond-only engine: conv_out writes v_c into the cond half of [0 | v_c], which any cfg_*_step with
+            # guidance 1 passes through exactly (0 + 1 (v_c - 0) = v_c)
+            self.model_pair = torch.zeros(2 * self.fl * h * w, 8, dtype=self.dtype, device=self.dev)
         self.sample: Optional[torch.Tensor] = None      # per-half fp32 sample for the plain forward() API path
         # frame-sharded window: R ranks (or an emulated R on one GPU) swap frame <-> pixel ownership around motion modules
         self.R = max(self.shard.group_size, self.shard.emulate_group)
         self.px = self.R > 1
         self.arena = None
         if self.px:
-            assert self.nb in (2, 3), "a frame shard holds every CFG half (the CFG combine stays rank-local)"
+            assert self.nb in (2, 3) or tuple(self.shard.halves) == (1,), \
+                "a frame shard holds every CFG half (the CFG combine stays rank-local), or the cond half alone"
             assert n_frames % self.R == 0 and self.fl == n_frames // self.R
             self._init_px()
 
@@ -346,7 +382,12 @@ class DenoiseEngine:
         The inputs always hold the two halves [uncond, cond].  An engine whose shard holds half 2 (three-branch CFG with
         a separate audio guidance scale) derives it from the cond half: the same image tokens, mask_cond_fea, masks,
         motion-frame features (bank half 1) and reference K/V, with the audio tokens set to zero -- the inputs training
-        saw when it dropped the audio alone."""
+        saw when it dropped the audio alone.  An engine of halves (1,) (the cond-only companion) takes the cond half alone.
+        The inputs are kept until the next window: a cond-only companion sets up its own window from them."""
+        self._window_args = dict(encoder_hidden_states=encoder_hidden_states, audio_embedding=audio_embedding,
+                                 mask_cond_fea=mask_cond_fea, full_mask=full_mask, face_mask=face_mask, lip_mask=lip_mask,
+                                 motion_scale=motion_scale, banks=banks, local_frames=local_frames)
+        self._window_gen += 1
         W, cfg, sh = self.W, self.cfg, self.shard
         dt, dev = self.dtype, self.dev
         halves, frames = list(sh.halves), list(sh.frames)
@@ -457,7 +498,7 @@ class DenoiseEngine:
 
     def set_schedule(self, timesteps: Sequence[int], coef: torch.Tensor, guidance: float, sampler: str = "ddim",
                      noise: Optional[torch.Tensor] = None, audio_guidance: Optional[float] = None,
-                     guidance_rescale: float = 0.0):
+                     guidance_rescale: float = 0.0, guided: Optional[Sequence[bool]] = None):
         """Per-window schedule.  The tables keep their device addresses (a captured graph reads them); the step count
         and the guidance scale are kernel ARGUMENTS of the captured launches and the sampler chooses the step kernel,
         so changing any of them drops the graph.  sampler "ddim": coef is the [n, 4] DDIM table
@@ -471,7 +512,11 @@ class DenoiseEngine:
         kernel argument of the captured graph too.
         guidance_rescale: phi in [0, 1] of guidance rescale (diffusers rescale_noise_cfg): the combined v is rescaled
         towards the window-wide std of v_c, v = phi v std(v_c) / std(v) + (1 - phi) v.  0 (the default) runs no extra
-        kernel; any other value is part of the captured graph as well."""
+        kernel; any other value is part of the captured graph as well.
+        guided: per-step bools of guidance limited to an interval (guided_steps), None for every step guided.  A step
+        marked False runs the cond-only companion (cond_engine): the UNet on the cond rows alone, then the sampler's
+        step on v = v_c.  Both share this engine's latents, sampler histories, step counter, tables and noise.  The
+        mask is not part of this engine's graph key: changing it never re-captures this engine."""
         n = len(timesteps)
         if n > self.MAX_STEPS:
             raise ValueError(f"{n} inference steps exceed the engine's schedule capacity ({self.MAX_STEPS})")
@@ -488,6 +533,12 @@ class DenoiseEngine:
         if audio_guidance is not None and not math.isfinite(audio_guidance):
             raise ValueError(f"audio_guidance must be finite, got {audio_guidance}")
         guidance_rescale = check_guidance_rescale(guidance_rescale)
+        if guided is not None:
+            guided = tuple(bool(g) for g in guided)
+            if len(guided) != n:
+                raise ValueError(f"guided has {len(guided)} entries for a {n}-step schedule")
+            if all(guided):
+                guided = None                            # every step guided: the path without an interval
         self.n_steps = n
         self.t_table[:n].copy_(torch.tensor([float(t) for t in timesteps], dtype=torch.float32))
         table = {"ddim": self.coef, "unipc": self.coef_uni}.get(sampler, self.coef_ms)
@@ -498,9 +549,53 @@ class DenoiseEngine:
         self.guidance_rescale = guidance_rescale
         if self.graph is not None and self._captured_with != self._schedule_key():
             self.graph = None
-        self.step_idx.zero_()
+        self.guided = guided
+        self.reset_steps()
         if noise is not None:
             self.set_noise(noise)
+        if self._window_args is not None:
+            self.cond_engine()                           # set up now, not inside the first unguided step
+
+    def reset_steps(self):
+        """Restart the schedule at step 0: the device step counter and the host-side one that picks each step's graph."""
+        self.step_idx.zero_()
+        self._next_step = 0
+
+    def cond_engine(self) -> Optional["DenoiseEngine"]:
+        """The cond-only companion of this engine when the schedule has an unguided step, else None.  It is an engine
+        of shard halves (1,) over the same frames and group, created on first use and kept.  Its latents, sampler
+        histories, step counter, t / coefficient tables and noise are this engine's tensors, at the same addresses, so
+        its graph and this engine's can be replayed in any order.  Its window follows this engine's last begin_window;
+        its step tail runs the sampler with guidance 1 on [0 | v_c]."""
+        if self.guided is None:
+            return None
+        if self._window_args is None:
+            raise RuntimeError("an unguided step needs this engine's window (begin_window) first")
+        c = self._cond
+        if c is None:
+            c = DenoiseEngine(self.W, self.h, self.w, self.f, replace(self.shard, halves=(1,)))
+            c.step_idx, c.t_table, c.coef, c.coef_ms, c.coef_uni = (self.step_idx, self.t_table, self.coef, self.coef_ms,
+                                                                   self.coef_uni)
+            c.latents, c.x0_hist, c.last_sample, c.x0_hist2 = self.latents, self.x0_hist, self.last_sample, self.x0_hist2
+            self._cond = c
+        if c._window_gen != self._window_gen:
+            c.begin_window(**self._window_args)
+            c._window_gen = self._window_gen
+        if c.noise is not self.noise:
+            c.noise, c.graph = self.noise, None
+        c.n_steps, c.sampler, c.guidance = self.n_steps, self.sampler, 1.0
+        if c.graph is not None and c._captured_with != c._schedule_key():
+            c.graph = None
+        return c
+
+    def release(self):
+        """Drop the captured graphs and close the peer arenas of this engine and its cond-only companion."""
+        for e in (self, self._cond):
+            if e is not None:
+                e.graph = None
+                if e.arena is not None:
+                    e.arena.close()
+        self._cond = None
 
     def _schedule_key(self):
         # the audio scale stays the last element
@@ -840,7 +935,7 @@ class DenoiseEngine:
                                 bias=W[f"{b.upsampler}.conv.b"])
         t = self.buf("out.gn", B * L0, c0)
         self._gn(x, "conv_norm_out", t, B, L0, cfg.norm_eps, True)
-        self.model_out = self.buf("out.conv", B * L0, 8)
+        self.model_out = self.model_pair[B * L0:] if self.nb == 1 else self.buf("out.conv", B * L0, 8)
         ops.conv3x3(t.view(B, h, w, c0), W["conv_out.w"], self.model_out, bias=W["conv_out.b"])
         return self.model_out
 
@@ -848,8 +943,10 @@ class DenoiseEngine:
     def _step_tail(self):
         """CFG combine + scheduler update (DDIM, DPM-Solver++ / Euler, Euler-a or UniPC) + step counter
         (face_animate.py:415-420).  Three branches or guidance rescale: a pre-pass writes the combined v as [0 | v] over
-        the first two halves, and the sampler's kernel then runs with guidance 1, which passes v through exactly."""
-        mo = self.model_out                    # every CFG half of the local frames: the combine is rank-local
+        the first two halves, and the sampler's kernel then runs with guidance 1, which passes v through exactly.  The
+        cond-only engine hands the sampler [0 | v_c] the same way (its guidance is 1)."""
+        # every CFG half of the local frames: the combine is rank-local
+        mo = self.model_pair if self.nb == 1 else self.model_out
         guidance = self.guidance
         if self.nb == 3 and self.audio_guidance is None:
             raise RuntimeError("a three-branch engine needs set_schedule(..., audio_guidance=) before it steps")
@@ -947,8 +1044,12 @@ class DenoiseEngine:
 
     @torch.no_grad()
     def step(self):
-        if self.graph is not None:
-            self.graph.replay()
+        """One denoising step: this engine's graph (or kernels), or the cond-only companion's on an unguided step."""
+        i = self._next_step
+        self._next_step = (i + 1) % self.n_steps
+        e = self if self.guided is None or self.guided[i] else self.cond_engine()
+        if e.graph is not None:
+            e.graph.replay()
         else:
-            self._forward()
-            self._step_tail()
+            e._forward()
+            e._step_tail()

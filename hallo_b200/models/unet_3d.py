@@ -219,7 +219,9 @@ class UNet3DConditionModel(nn.Module):
         """The denoising engine of this window geometry.  branches = 3 (no shard given) builds an engine with the CFG
         halves (0, 1, 2) for a separate audio guidance scale; a shard brings its own halves.  Engines of the same
         geometry and frames that differ only in their halves replace each other: switching between two and three
-        branches keeps one set of activation buffers alive (the three-branch set is about 1.5x the two-branch one)."""
+        branches keeps one set of activation buffers alive (the three-branch set is about 1.5x the two-branch one).
+        The cond-only companion that runs the unguided steps of a guidance interval belongs to its engine
+        (DenoiseEngine.cond_engine), not to this cache: it lives and goes with that engine."""
         if shard is None and branches == 3:
             shard = Shard(halves=(0, 1, 2), frames=tuple(range(n_frames)))
         elif branches not in (2, 3) or (shard is not None and len(shard.halves) != branches):
@@ -232,9 +234,7 @@ class UNet3DConditionModel(nn.Module):
             for k in [k for k, e in self._engines.items()
                       if k[:3] == (h, w, n_frames) and tuple(e.shard.frames) == frames and e.nb != branches]:
                 old = self._engines.pop(k)
-                old.graph = None
-                if old.arena is not None:
-                    old.arena.close()
+                old.release()                    # its cond-only companion (guidance_interval) goes with it
                 del old
             eng = DenoiseEngine(W, h, w, n_frames, shard)
             self._engines[key] = eng
