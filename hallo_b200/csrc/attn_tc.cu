@@ -286,9 +286,7 @@ static int launch_attn(const hb_attention_params* q, cudaStream_t stream) {
   if ((rc = make_qkv_map(&tmQ, q->dtype, q->Q, D, q->heads, q->L, q->frames, q->ldq, 128))) return rc;
   if ((rc = make_qkv_map(&tmK0, q->dtype, q->K, D, q->heads, q->L, q->frames, q->ldk, BN))) return rc;
   if ((rc = make_qkv_map(&tmV0, q->dtype, q->V, D, q->heads, q->L, q->frames, q->ldv, BN))) return rc;
-  if (q->ref_index != nullptr) {
-    if (q->Kref == nullptr || q->Vref == nullptr || q->ref_frames <= 0)
-      return fail(HB_ERR_NULL, "attention: ref_index given without Kref/Vref");
+  if (q->ref_index != nullptr) {     // Kref / Vref / ref_frames checked by hallo_b200_attention
     if ((rc = make_qkv_map(&tmK1, q->dtype, q->Kref, D, q->heads, q->L, q->ref_frames, q->ldkref, BN))) return rc;
     if ((rc = make_qkv_map(&tmV1, q->dtype, q->Vref, D, q->heads, q->L, q->ref_frames, q->ldvref, BN))) return rc;
   } else {

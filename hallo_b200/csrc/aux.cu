@@ -1262,6 +1262,11 @@ extern "C" int hallo_b200_cross_attention(int dtype, const void* Q, int64_t ldq,
   if (head_dim % 8 || (n_keys != 4 && n_keys != 32) || ldq % 8 || ldkv % 8 || ldo % 8 ||
       q_region_stride % 8 || kv_region_stride % 8 || o_region_stride % 8)
     return fail(HB_ERR_BAD_SHAPE, "cross_attention: head_dim=%d n_keys=%d", head_dim, n_keys);
+  // The CUDA-core kernel reads Q and stores O 8 elements at a time (16 bytes), the tensor-core kernel stores O as
+  // 32-bit pairs.  Misaligned Q / O are rejected rather than sent to either path, so that the "xattn_tc" option never
+  // decides whether a call works.
+  if ((reinterpret_cast<uintptr_t>(Q) | reinterpret_cast<uintptr_t>(O)) & 15)
+    return fail(HB_ERR_BAD_SHAPE, "cross_attention: Q %p and O %p must be 16-byte aligned", Q, O);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   {
     // tensor-core path (csrc/attn_tc.cu) for the layouts the engine produces; CUDA cores otherwise

@@ -190,6 +190,9 @@ int hallo_b200_gemm_choose_splits(int tiles, int sm_units, int K, int cta_group,
  *             frames, -1 for uncond frames -- SURVEY quirk Q9).  NULL = plain self-attention.
  *   O       : [frames*L, ldo], same head layout.
  *   head_dim in {40, 80, 160, 512}; scale = head_dim^-0.5; no mask, no dropout.  Scores and softmax in fp32.
+ *   Checked before anything runs: Q, K, V, O non-NULL, and Kref, Vref non-NULL with ref_frames >= 1 when ref_index
+ *             is given (HB_ERR_NULL); 1 <= heads <= 256, L >= 1, frames >= 1, every ld* a multiple of 8, Q / K / V /
+ *             Kref / Vref 16-byte aligned, O 4-byte aligned (the kernels store O as 32-bit pairs) (HB_ERR_BAD_SHAPE).
  *   head_dim 512 (the VAE mid-block attention, diffusers Attention(heads=1) over the (h/8)(w/8) tokens of a frame):
  *             heads == 1 and no reference keys; L may be any length.  The V / O columns are split over 4 CTAs of
  *             128 columns, each of which recomputes the 512-wide Q K^T.
@@ -239,7 +242,9 @@ int hallo_b200_groupnorm(int dtype, const void* x1, int C1, const void* x2, int 
 /* softmax(q k^T / sqrt d) v against n_keys in {4, 32} keys per (kv-frame, head, region):
  * image-token cross-attention (mutual_self_attention.py:289-303) and the three audio cross-attentions
  * (attention.py:854-890).  Frame n reads keys of kv-frame n / kv_frame_div.  Region r reads Q columns
- * at r*q_region_stride, K/V columns at r*kv_region_stride, writes O columns at r*o_region_stride. */
+ * at r*q_region_stride, K/V columns at r*kv_region_stride, writes O columns at r*o_region_stride.
+ * Q and O must be 16-byte aligned (the CUDA-core kernel moves 8 elements per access); otherwise HB_ERR_BAD_SHAPE,
+ * whichever kernel the "xattn_tc" option selects. */
 int hallo_b200_cross_attention(int dtype, const void* Q, int64_t ldq, int q_region_stride, const void* K,
                                const void* V, int64_t ldkv, int kv_region_stride, void* O, int64_t ldo,
                                int o_region_stride, int frames, int L, int heads, int head_dim, int n_keys,
